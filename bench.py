@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the B200-native Epsilla vector-search hot path.
+"""bench.py — headline benchmark of the H100-native Epsilla vector-search hot path.
 
 Metric (BASELINE.json): QPS at recall@10 >= 0.99 on 10M x 768 float32, batch = 1024, top-10, reported with the
 roofline fraction of the dominant kernel and with the reference's own CPU path timed on the same box.
 
-  python bench.py [--gpus N --steps K --warmup W] [--impl reference]
+  python bench.py [--gpus N --steps K --warmup W] [--impl reference] [--dump-outputs DIR]
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Workload.  Three synthetic 10M x 768 tables (random floats, seeded, generated on the device):
@@ -24,14 +24,15 @@ Workload.  Three synthetic 10M x 768 tables (random floats, seeded, generated on
     with the exact scan.
 `value` is the fastest mode (graph at the smallest L of the sweep that reaches the target, or the exact scan) with
 recall@10 >= 0.99 on the --dist table; --extra-tables measures the other tables in the same run (N = 1) and prints
-them as "uniform" / "cluster" records with their own recall, QPS and rooflines.  The default run (3 min) carries
-the uniform record; `--extra-tables cluster,uniform` (5.7 min: one more graph build) adds the isotropic one, as in
-profiles/r02_bench_10Mx768_manifold_3lanes_*final.json.log.
+them as "uniform" / "cluster" records with their own recall, QPS and rooflines.  The default run carries the uniform
+record; `--extra-tables cluster,uniform` (one more graph build) adds the isotropic one.
 
 One "step" = one pass of the hot path over one batch of 1024 queries per GPU.  A step is timed with CUDA events on
 the index's launch stream, bracketed by barrier + synchronize, MAX over ranks.  `value` has the queries already
 resident in HBM; `e2e` goes through the host-buffer C-ABI call (eps_search_batch: H2D of the queries and D2H of
-ids / distances / counts inside the timed region).
+ids / distances / counts inside the timed region).  --dump-outputs DIR writes what the last timed step of `value`
+returned (ids and counts as float64, distances as float32) to DIR/<name>.npy; the inputs are seeded, so two builds run
+with the same arguments can be compared output for output.
 
 Reference arm (--impl reference) and `cpu_baseline`: the reference's own VecSearchExecutor (oracle/_ref = its
 sources compiled unmodified) searching THE SAME CSR graph at the same queue length on the host cores, in the two
@@ -46,6 +47,7 @@ ROWS (config C5 shape): every rank searches the same batch over its shard and th
 the library itself (eps_search_batch_sharded: ncclAllGather + merge kernel on the index stream).
 """
 import argparse
+import atexit
 import json
 import os
 import subprocess
@@ -86,8 +88,7 @@ def parse():
     p.add_argument("--knn-k", type=int, default=64)
     p.add_argument("--nnd-iters", type=int, default=14)
     p.add_argument("--extra-tables", default="uniform", help="other SURVEY 8d tables measured in the same run at N=1 "
-                   "(uniform: exact scan, + graph with --uniform-graph; cluster: graph build + graph + exact scan, +2.7 min — "
-                   "the committed logs under profiles/ were made with 'cluster,uniform'); '' = none")
+                   "(uniform: exact scan, + graph with --uniform-graph; cluster: graph build + graph + exact scan); '' = none")
     p.add_argument("--uniform-graph", action="store_true", help="also build + search a graph on the iid-uniform table")
     p.add_argument("--shard-rows", action="store_true")
     p.add_argument("--recall-target", type=float, default=0.99)
@@ -99,6 +100,7 @@ def parse():
     p.add_argument("--filter", default="", help="(reference-child) filter string for the reference's parser")
     p.add_argument("--attr-mod", type=int, default=0, help="(reference-child) INT4 column ID = row %% this")
     p.add_argument("--seed-shift", type=int, default=0, help="(reference-child) table seed = 42 + this (row shards)")
+    p.add_argument("--dump-outputs", default="", metavar="DIR", help="write the outputs of the last timed step to DIR/<name>.npy")
     return p.parse_args()
 
 
@@ -146,15 +148,25 @@ def _draw(out, dist, g, device, centers, umap):
     out.addmm_(z, umap)
 
 
-def gen_table(rows, dim, dist, seed, device, centers_n=1024):
+def table_chunks(rows, dim, dist, seed, device, centers_n=1024, out=None):
+    """The rows of the seeded table in 1M-row chunks, drawn in order (into `out` when given): (first row, chunk)."""
     import torch
     g = torch.Generator(device=device)
     g.manual_seed(seed)
-    X = torch.empty((rows, dim), dtype=torch.float32, device=device)
     centers, umap = (None, None) if dist == "uniform" else _mixture(dim, dist, device, centers_n)
     step = 1_000_000
     for r0 in range(0, rows, step):
-        _draw(X[r0:min(rows, r0 + step)], dist, g, device, centers, umap)
+        n = min(rows, r0 + step) - r0
+        buf = out[r0:r0 + n] if out is not None else torch.empty((n, dim), dtype=torch.float32, device=device)
+        _draw(buf, dist, g, device, centers, umap)
+        yield r0, buf
+
+
+def gen_table(rows, dim, dist, seed, device, centers_n=1024):
+    import torch
+    X = torch.empty((rows, dim), dtype=torch.float32, device=device)
+    for _ in table_chunks(rows, dim, dist, seed, device, centers_n, out=X):
+        pass
     return X
 
 
@@ -169,7 +181,7 @@ def gen_queries(n, dim, dist, seed, device, centers_n=1024):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read only; the sampler is stopped at exit)."""
 
     def __init__(self, index):
         self.index = index
@@ -184,6 +196,7 @@ class ClockSampler:
             self.proc = subprocess.Popen(["nvidia-smi", "-i", str(self.index), "--query-gpu=" + q,
                                           "--format=csv,noheader,nounits", "-lms", "100"],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
+            atexit.register(self.proc.kill)
             self.t = threading.Thread(target=self._read, daemon=True)
             self.t.start()
         except Exception:
@@ -218,14 +231,16 @@ class ClockSampler:
 
 
 def measured_peaks():
+    """HBM GB/s and dense BF16 TFLOP/s to state rooflines against: MEASURED_PEAKS.json when present, else the H100 SXM
+    data sheet (3.35 TB/s, 989 TFLOP/s at 700 W; a card with a lower power limit does not reach them)."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         try:
             d = json.load(open(p))
-            return float(d["hbm_gbs"]), float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1590.0))), "measured"
+            return float(d["hbm_gbs"]), float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 989.0))), "measured"
         except Exception:
             pass
-    return 6650.0, 1590.0, "fallback"
+    return 3350.0, 989.0, "H100 SXM data sheet"
 
 
 def workload_name(a, extra=""):
@@ -247,9 +262,13 @@ def reference_child(a):
     from oracle import oracle
     g = np.load(a.graph_file, allow_pickle=False)
     dev = "cuda:0" if torch.cuda.is_available() else "cpu"
-    X = gen_table(a.rows, a.dim, a.dist, 42 + a.seed_shift, dev, a.centers)
-    if a.metric == "cosine":
-        X /= X.norm(dim=1, keepdim=True)
+
+    def host_table(dst):
+        # chunk by chunk: the parent's table and index stay resident on the same GPU meanwhile
+        for r0, c in table_chunks(a.rows, a.dim, a.dist, 42 + a.seed_shift, dev, a.centers):
+            if a.metric == "cosine":
+                c /= c.norm(dim=1, keepdim=True)
+            dst[r0:r0 + c.shape[0]] = c.cpu().numpy()
     cores = os.cpu_count() or 1
     kind = "reference" if oracle.have_ref() else "port"
     n_indexed = int(g["n_indexed"])
@@ -257,7 +276,8 @@ def reference_child(a):
     out = {"kind": kind, "cores": cores, "L": L, "graph": n_indexed > 0, "modes": {}}
     queries = g["queries"]  # [steps_total, nq, dim]
     if kind != "reference":
-        Xh = X.cpu().numpy()
+        Xh = np.empty((a.rows, a.dim), np.float32)
+        host_table(Xh)
         port = oracle.Port()
         vals = []
         for s in range(queries.shape[0]):
@@ -271,10 +291,7 @@ def reference_child(a):
         print(json.dumps(out))
         return
     r = oracle.Ref(a.metric, a.dim, a.rows, [("ID", "int4")])
-    step = 1_000_000
-    for r0 in range(0, a.rows, step):  # device -> the reference's own table, chunked (no second 30 GB host copy)
-        r.vectors[r0:min(a.rows, r0 + step)] = X[r0:r0 + step].cpu().numpy()
-    del X
+    host_table(r.vectors)  # straight into the reference's own table (no second host copy)
     r.set_row_count(a.rows)
     if a.attr_mod > 0:
         r.set_attr_column("ID", (np.arange(a.rows) % a.attr_mod).astype(np.int32))
@@ -617,7 +634,7 @@ def main():
         A.set_mode(m)
         A.search(A.Qpool[0])
         rec = recall_of(A.truth, A.out_ids, a.k)
-        if m[0] == "graph" and a.width > 1:  # wide mode is not bit-reproducible: the gate is the worse of two passes
+        if m[0] == "graph" and a.width > 1:  # the gate is the worse of two passes
             A.search(A.Qpool[0])
             rec = min(rec, recall_of(A.truth, A.out_ids, a.k))
         # every rank builds its own graph (NN-descent is not deterministic): the gate is the worst rank's recall, so that
@@ -665,6 +682,10 @@ def main():
     ms_serial, stats = timed_device_steps(mode, a.steps, a.warmup)
     if prof_region:
         torch.cuda.profiler.stop()
+    if group is not None:
+        last_out = {"ids": m_ids.cpu().numpy(), "distances": m_d.cpu().numpy()}
+    else:
+        last_out = {"ids": A.out_ids.cpu().numpy(), "distances": A.out_d.cpu().numpy(), "counts": A.out_c.cpu().numpy()}
     if stats[0] is None:  # row shards: the sharded call returns no counters; the local search of the same steps does
         stats = [A.search(A.Qpool[(a.warmup + s_) % n_pool], want_stats=True) for s_ in range(a.steps)]
         for st_ in stats:
@@ -685,6 +706,8 @@ def main():
         timed_overlapped(mode, max(a.warmup, len(A.lanes)), 0)
         ms_dev = timed_overlapped(mode, a.steps, a.warmup)
         n_lanes = len(A.lanes)
+        ln = A.lanes[(a.steps - 1) % n_lanes]  # the lane that ran the last step
+        last_out = {"ids": ln["ids"].cpu().numpy(), "distances": ln["d"].cpu().numpy(), "counts": ln["c"].cpu().numpy()}
         kernel_ms = ms_dev  # region time: the launches of different lanes overlap, per-launch times do not add up
 
     # ---- e2e: host buffers through the public C-ABI call, H2D + D2H inside the timed region ----
@@ -767,24 +790,15 @@ def main():
                     "kernel": "bf_dist_tile_kernel + bf_select_kernel", "peak_source": peak_src, "kernel_ms_per_step": k_ms / n_steps}
         flop = n_steps * rows * float(a.batch) * a.dim * 2.0
         ach = flop / (k_ms / 1000.0) / 1e12 if k_ms > 0 else 0.0
-        peak = tf_peak / 2.0 if coarse == "tf32" else tf_peak  # tcgen05 kind::tf32 runs at half the bf16 rate
+        peak = tf_peak / 2.0 if coarse == "tf32" else tf_peak  # wgmma TF32 runs at half the BF16 rate
         return {"bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "traffic": None,
-                "kernel": "tc_dist_kernel (tcgen05 kind::%s, fused threshold select) + bf_select_kernel + rescore_kernel" % (
-                    "tf32" if coarse == "tf32" else "f16/bf16"),
-                "peak_source": "%s bf16 sustained (%.0f TF/s)%s" % (peak_src, tf_peak, " / 2 for TF32" if coarse == "tf32" else ""),
+                "kernel": "tc_dist_kernel (wgmma %s, fused threshold select) + bf_select_kernel + rescore_kernel" % (
+                    "tf32" if coarse == "tf32" else "bf16"),
+                "peak_source": "%s bf16 (%.0f TF/s)%s" % (peak_src, tf_peak, " / 2 for TF32" if coarse == "tf32" else ""),
                 "kernel_ms_per_step": k_ms / n_steps,
                 "hbm_algorithmic_GBps": bytes_alg / (k_ms / 1000.0) / 1e9 if k_ms > 0 else 0.0}
 
     roof = graph_roofline(agg, mode[1], kernel_ms, a.steps) if mode[0] == "graph" else scan_roofline(mode[2], kernel_ms, a.steps)
-    if mode[0] == "graph":  # measured DRAM traffic of this exact workload, when an ncu capture of it is committed
-        try:
-            with open(os.path.join(ROOT, "profiles", "r02_measured_traffic.json")) as f:
-                for e in json.load(f)["entries"]:
-                    if (e["rows"], e["dim"], e["dist"], e["batch"], e["L"], e["width"]) == (a.rows, a.dim, a.dist, a.batch, mode[1], a.width):
-                        roof["traffic"] = e["bytes_per_launch"]
-                        roof["traffic_source"] = e["source"]
-        except (OSError, ValueError, KeyError):
-            pass
 
     # ---- secondary records of the non-chosen modes, each with its own roofline ----
     extra = {}
@@ -817,7 +831,7 @@ def main():
         "dtype": "f32", "data": "synthetic",
         "config": {"workload": workload_name(a, ", mode=%s; %s" % (
             ("graph search L=%d width=%d" % (mode[1], a.width)) if mode[0] == "graph" else
-            "exact scan (tcgen05 %s coarse pass + fp32 re-score)" % mode[2],
+            "exact scan (wgmma %s coarse pass + fp32 re-score)" % mode[2],
             "row shards + in-library ncclAllGather + merge" if a.shard_rows else "replicated table, query stream partitioned over ranks")),
             key_rec: chosen[key_rec], "l2_flush": "inputs (%.1f GB table) larger than L2" % (rows * a.dim * 4 / 1e9),
             "fp64_groundtruth_check": chk, "batches_in_flight": n_lanes},
@@ -931,6 +945,10 @@ def main():
         except Exception as e:
             out[t] = {"failed": repr(e)}
     if rank == 0:
+        if a.dump_outputs:
+            os.makedirs(a.dump_outputs, exist_ok=True)
+            for name, arr in last_out.items():
+                np.save(os.path.join(a.dump_outputs, name + ".npy"), arr.astype(np.float32 if name == "distances" else np.float64))
         print(json.dumps(out))
     if group is not None:
         group.close()

@@ -1,5 +1,5 @@
 /*
- * epsilla_b200.h — C ABI of libepsilla_b200.so, the B200-native (sm_100a) implementation of
+ * epsilla_b200.h — C ABI of libepsilla_b200.so, the H100-native (sm_90a) implementation of
  * Epsilla's vector-search hot path.  POD-only: plain pointers and sizes, no C++/torch types.
  *
  * Every entry point cites the reference interface it replaces (paths relative to
@@ -164,17 +164,17 @@ EPS_API int eps_index_config(eps_index* ix, int64_t L_master, int64_t L_local, i
 /* Graph-search expansion width: how many unchecked queue entries are expanded per iteration.  1 (default)
  * reproduces the reference at IntraQueryThreads = 1 exactly; 2 .. 8 are the device analogue of the reference's
  * IntraQueryThreads > 1 (config.hpp:18, default 4): candidates expanded in parallel against a slightly stale
- * bound — higher throughput, results not bit-identical to the sequential order (as in the reference). */
+ * bound — higher throughput, results not bit-identical to the sequential order (as in the reference) but the same on
+ * every run. */
 EPS_API int eps_index_set_search_width(eps_index* ix, int width);
 
-/* Launch geometry of the graph-search kernel (performance knob, never changes results in width 1 and only the
- * usual run-to-run variation of the wide mode otherwise): ring_slots = shared-memory row slots per CTA that TMA
+/* Launch geometry of the graph-search kernel (performance knob, never changes results): ring_slots = shared-memory row slots per CTA that TMA
  * bulk copies land in (0 = auto: ~48 KB of rows), ctas_per_sm = cap on resident CTAs, i.e. in-flight queries, per SM
  * (0 = whatever fits).  No reference counterpart (the CPU executor has no such geometry). */
 EPS_API int eps_index_set_graph_tuning(eps_index* ix, int ring_slots, int ctas_per_sm);
 
 /* Precision of the COARSE pass of large-batch exact scans (nq >= 64): 0 = none (fp32 SIMT tiles only),
- * 1 = tcgen05 kind::tf32 on the fp32 rows (default), 2 = tcgen05 kind::f16 on a bf16 mirror of the table
+ * 1 = wgmma TF32 on the fp32 rows (default), 2 = wgmma BF16 on a bf16 mirror of the table
  * (+50 % HBM).  Whatever the mode, the k' = k + max(118, k) best coarse candidates of every query are re-evaluated
  * with the exact fp32 direct form, so returned distances are fp32-exact, and a GUARD checks that no row outside
  * the candidate list can belong to the answer: with T = the k'-th best coarse distance, e_k = the exact k-th best

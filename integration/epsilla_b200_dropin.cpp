@@ -11,7 +11,7 @@
 // Everything else of the class (SearchByAttribute, the public result arrays search_result_ / distance_ /
 // dimension_ that TableMVP::Search reads after the call — engine/db/table_mvp.cpp:365-394) stays the
 // reference's.  TableMVP, ExecutorPool, DBServer and the filter parser therefore run unchanged; the dense
-// vector search and the graph build run on the B200 through include/epsilla_b200.h.
+// vector search and the graph build run on the GPU through include/epsilla_b200.h.
 //
 // State: one device mirror (eps_index) per (vector table, graph, executor parameters), shared by the
 // NumExecutorPerField executors TableMVP creates for a field (engine/db/table_mvp.cpp:72-89) and destroyed

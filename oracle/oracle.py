@@ -2,7 +2,7 @@
 
 ``Port``  : oracle/_ref/libepsilla_port.so  (oracle_port.c, the plain-C restatement; always buildable)
 ``Ref``   : oracle/_ref/libepsilla_ref.so   (the reference's own sources compiled unmodified;
-            built only where /root/reference exists, but the .so travels to the GPU box)
+            built only where reference_dir() finds a checkout of the reference)
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / ``--impl reference`` legs import
 this module.  The product package (vectordb_b200) never does.
@@ -25,13 +25,23 @@ FIELD_NP = {"int1": np.int8, "int2": np.int16, "int4": np.int32, "int8": np.int6
             "double": np.float64, "bool": np.uint8}
 
 
+DEFAULT_REFERENCE = "/root/reference"
+
+
+def reference_dir():
+    """Checkout of epsilla-cloud/vectordb to compile the reference oracle from: $EPSILLA_REFERENCE, else
+    DEFAULT_REFERENCE; None when neither holds the reference's engine/ sources."""
+    d = os.environ.get("EPSILLA_REFERENCE") or DEFAULT_REFERENCE
+    return d if os.path.isdir(os.path.join(d, "engine")) else None
+
+
 def build(force=False):
-    """Compile the port (always) and the reference library (when /root/reference is present)."""
+    """Compile the port (always) and the reference library (when reference_dir() finds the reference)."""
     if force or not os.path.exists(PORT_SO) or os.path.getmtime(PORT_SO) < os.path.getmtime(
             os.path.join(HERE, "oracle_port.c")):
         subprocess.check_call(["make", "-C", HERE, "port"], stdout=subprocess.DEVNULL)
-    if os.path.isdir("/root/reference/engine") and (force or not os.path.exists(REF_SO)):
-        subprocess.check_call(["make", "-C", HERE, "ref", "-j8"], stdout=subprocess.DEVNULL)
+    if reference_dir() and (force or not os.path.exists(REF_SO)):
+        subprocess.check_call(["make", "-C", HERE, "ref", "-j8", "REF=" + reference_dir()], stdout=subprocess.DEVNULL)
 
 
 def have_ref():
@@ -150,12 +160,12 @@ class Ref:
 
     def __init__(self, metric, dim, capacity, attr_cols=(), lib_path=None):
         """attr_cols: sequence of (name, type) with type in FIELD_TYPE.  lib_path: an alternative build of the
-        same driver (integration/_build/libepsilla_ref_b200.so = the reference engine with the GPU drop-in)."""
+        same driver (oracle/_ref/dropin/libepsilla_ref_b200.so = the reference engine with the GPU drop-in)."""
         if lib_path is None:
             if not have_ref():
                 build()
             if not have_ref():
-                raise RuntimeError("oracle/_ref/libepsilla_ref.so not available (no /root/reference here and no prebuilt)")
+                raise RuntimeError("oracle/_ref/libepsilla_ref.so not available (no reference checkout found to build it from)")
         L = C.CDLL(lib_path or REF_SO)
         L.ref_create.restype = C.c_void_p
         L.ref_create.argtypes = [C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]

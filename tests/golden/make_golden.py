@@ -1,8 +1,8 @@
 """Generate the committed golden fixtures from the REFERENCE ITSELF (oracle/_ref/libepsilla_ref.so =
 epsilla-cloud/vectordb's own hot-path sources compiled unmodified, see oracle/Makefile).
 
-Run in the build container (needs /root/reference):   python tests/golden/make_golden.py
-The GPU box has no /root/reference; tests read only the .npz files written here.
+Run where oracle.reference_dir() finds a checkout of the reference:   python tests/golden/make_golden.py
+The tests read only the .npz files written here.
 
 Fixtures
   dense_vector.npz  engine/test/engine/db/db_server.cpp:92-319  (DbServer.DenseVector) + :1407-1630 (DenseVectorFilter)
@@ -16,11 +16,13 @@ Fixtures
 """
 import os
 import sys
+import zlib
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
 from oracle.oracle import Ref  # noqa: E402
 
 OUT = os.path.dirname(os.path.abspath(__file__))
@@ -164,6 +166,11 @@ def rand2k():
         r.set_graph(0, np.zeros(1, np.int64), np.zeros(0, np.int64), 0)
         r.set_row_count(400)
         run("brute10", 10)
+    # the l2 / ip table is X itself: stored as its CRC (tests/conftest.py redraws it) to keep the fixture small
+    assert np.array_equal(out["stored_l2"], X) and np.array_equal(out["stored_ip"], X)
+    for key in ("X", "stored_l2", "stored_ip"):
+        del out[key]
+    out["table_crc32"] = np.int64(zlib.crc32(X.tobytes()))
     np.savez_compressed(os.path.join(OUT, "rand2k.npz"), **out)
 
 
@@ -197,9 +204,104 @@ def refgraph20k():
     np.savez_compressed(os.path.join(OUT, "refgraph20k.npz"), **out)
 
 
+def refchecks():
+    """What the reference itself answers for the CPU checks of tests/test_oracle.py: distance kernels and Normalize,
+    the Expr evaluator on a typed attribute table, and VecSearchExecutor::Search (T = 1) on a graph it built."""
+    from helpers import gen
+    out = {}
+    rng = np.random.default_rng(7)
+    dims = list(range(1, 40)) + [127, 128, 130, 131, 768, 769, 770, 771, 1536]
+    dist = []
+    for d in dims:
+        r = {m: Ref(m, d, 4) for m in ("l2", "ip", "cosine")}
+        for _ in range(4):
+            a, b = rng.standard_normal(d).astype(np.float32), rng.random(d, dtype=np.float32)
+            dist.append([r[m].distance(a, b) for m in ("l2", "ip", "cosine")])
+    out["dist"] = np.array(dist, np.float32)  # [len(dims) * 4, 3 metrics], drawn in that order
+    a = rng.random(333, dtype=np.float32)
+    out["normalized"] = r["l2"].normalize(a)
+
+    rng = np.random.default_rng(3)
+    n = 64
+    r = Ref("l2", 4, n, [("a", "int1"), ("b", "int2"), ("c", "int4"), ("d", "int8"), ("x", "float"), ("y", "double"),
+                         ("t", "bool")])
+    r.set_rows(rng.random((n, 4), dtype=np.float32))
+    r.set_attr_column("a", rng.integers(-100, 100, n)); r.set_attr_column("b", rng.integers(-1000, 1000, n))
+    r.set_attr_column("c", rng.integers(-10**6, 10**6, n)); r.set_attr_column("d", rng.integers(-10**12, 10**12, n))
+    r.set_attr_column("x", rng.standard_normal(n)); r.set_attr_column("y", rng.standard_normal(n))
+    r.set_attr_column("t", rng.integers(0, 2, n))
+    out["fe_attrs"], out["fe_stride"] = r.attrs.copy(), np.int64(r.stride)
+    out["fe_exprs"] = np.array(FILTER_EVAL_EXPRS)
+    res = np.zeros((len(FILTER_EVAL_EXPRS), n, 2), np.int8)
+    for i, e in enumerate(FILTER_EVAL_EXPRS):
+        out["fe_nodes_%d" % i] = r.filter_nodes(e)
+        for row in range(n):
+            for j, dd in enumerate((0.25, 0.75)):
+                res[i, row, j] = r.filter_eval(e, row, dd)
+    out["fe_result"] = res
+
+    n, d = 3000, 24
+    X, Q = gen(n, d, 5), gen(12, d, 6)
+    r = Ref("l2", d, n, [("ID", "int4")])
+    r.set_rows(X)
+    r.set_attr_column("ID", np.arange(n))
+    ni, off, nb, nav = r.build(threads=2)
+    r.make_executors(1, 1, 500, counting=True)
+    out.update(live_n_indexed=np.int64(ni), live_offsets=off.astype(np.int64), live_nbrs=nb.astype(np.int32),
+               live_nav=np.int64(nav), live_attrs=r.attrs.copy(), live_stride=np.int64(r.stride))
+    for fi, f in enumerate(LIVE_FILTERS):
+        out["live_nodes_%d" % fi] = r.filter_nodes(f)
+        ids = np.full((len(Q), 20), -1, np.int64)
+        ds = np.full((len(Q), 20), np.inf, np.float64)
+        cnt, nd = np.zeros(len(Q), np.int64), np.zeros(len(Q), np.int64)
+        for qi, q in enumerate(Q):
+            a, b, c = r.search(q, 20, f)
+            ids[qi, :len(a)], ds[qi, :len(a)], cnt[qi], nd[qi] = a, b, len(a), c
+        out["live_ids_%d" % fi], out["live_dists_%d" % fi], out["live_counts_%d" % fi], out["live_ndist_%d" % fi] = ids, ds, cnt, nd
+    np.savez_compressed(os.path.join(OUT, "refchecks.npz"), **out)
+
+
+def facets():
+    """FacetExecutor::Aggregate + Project of the reference over exact top-64 result lists (tests/test_gpu_parity.py
+    test_facets_match_reference): the attribute table, the parsed value expressions and the JSON the reference returns."""
+    import json
+    from helpers import gen
+    from oracle.oracle import Port
+    n, d, nq, k = 4000, 16, 12, 64
+    X, Q = gen(n, d, 111), gen(nq, d, 112)
+    rng = np.random.default_rng(113)
+    r = Ref("l2", d, n, FACET_COLS)
+    r.set_rows(X)
+    idv, wv, fv = np.arange(n), rng.random(n), rng.integers(0, 2, n)
+    names = ["n%d" % v for v in rng.integers(0, 9, n)]
+    for nm, v in (("ID", idv), ("w", wv), ("flag", fv)):
+        r.set_attr_column(nm, v)
+    r.set_string_column("name", names)
+    ids, ds, cnt, _ = Port().search_batch(metric="l2", vectors=X, queries=Q, limit=k, L=500, prefilter=True)
+    out = {"attrs": r.attrs[: n * r.stride].copy(), "stride": np.int64(r.stride), "name_offset": np.int64(r.attr_offset("name")),
+           "ids": ids, "dists": ds, "counts": cnt}
+    for ci, (group, aggs) in enumerate(FACET_CASES):
+        out["key_nodes_%d" % ci], kt = r.value_nodes(group if group else "1")
+        out["key_type_%d" % ci] = np.int64(kt)
+        for ai, a in enumerate(aggs):
+            inner = "1" if a.upper().startswith("COUNT(") else a[a.index("(") + 1:-1]
+            out["agg_nodes_%d_%d" % (ci, ai)] = r.value_nodes(inner)[0]
+        out["want_%d" % ci] = np.array(json.dumps([r.facet(group, aggs, ids[q, :cnt[q]], ds[q, :cnt[q]]) for q in range(nq)]))
+    np.savez_compressed(os.path.join(OUT, "facets.npz"), **out)
+
+
+FILTER_EVAL_EXPRS = ["a < 0", "b >= 10 OR c < 0", "d / 1000 > a * b", "x + y < 0.5", "t = true", "NOT t = false", "t",
+                     "NOT (a > 3 AND t = true)", "c % 5 = 2", "@distance < 0.5", "@distance < 0.5 AND a < 1000",
+                     "x * @distance > y", "(a + b) * 2 - c / 3 <= d", "a = b OR x <> y", "true", "false OR t"]
+LIVE_FILTERS = ["", "ID >= 1500", "@distance > 1.0"]
+FACET_COLS = [("ID", "int4"), ("w", "double"), ("flag", "bool"), ("name", "string")]
+FACET_CASES = [("ID % 7", ["SUM(w)", "COUNT(*)", "MIN(ID)", "MAX(w * 2 + @distance)"]), ("name", ["COUNT(*)", "SUM(ID)"]),
+               ("flag", ["COUNT(*)", "MAX(@distance)"]), ("w * 2", ["COUNT(*)"]), ("", ["COUNT(*)", "SUM(w)", "MIN(@distance)"])]
+
+
 if __name__ == "__main__":
     only = sys.argv[1:]
-    for fn in (dense_vector, halfcircle, rand2k, refgraph20k):
+    for fn in (dense_vector, halfcircle, rand2k, refgraph20k, refchecks, facets):
         if not only or fn.__name__ in only:
             fn()
     for f in sorted(os.listdir(OUT)):

@@ -88,12 +88,12 @@ def test_header_is_plain_c(tmp_path):
 
 
 def test_dropin_library_binds_reference_symbols_to_the_gpu_path():
-    """integration/_build/libepsilla_ref_b200.so = the reference's own objects with three symbols replaced: each must be
+    """oracle/_ref/dropin/libepsilla_ref_b200.so = the reference's own objects with three symbols replaced: each must be
     defined exactly once (strong), and the library must import the C ABI from libepsilla_b200.so (no CPU body left)."""
     import subprocess
-    so = os.path.join(ROOT, "integration", "_build", "libepsilla_ref_b200.so")
+    so = os.path.join(ROOT, "oracle", "_ref", "dropin", "libepsilla_ref_b200.so")
     if not os.path.exists(so):
-        pytest.skip("drop-in not built (needs /root/reference at build time)")
+        pytest.skip("drop-in not built (needs a reference checkout at build time)")
     dyn = subprocess.check_output(["nm", "-D", "-C", so], text=True)
     for sym in ("VecSearchExecutor::Search(", "VecSearchExecutor::VecSearchExecutor(long, long,",
                 "ANNGraphSegment::BuildFromVectorTable("):

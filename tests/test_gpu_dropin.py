@@ -1,7 +1,7 @@
 """GPU test of the drop-in boundary: the reference engine's OWN classes (TableSegmentMVP, ANNGraphSegment,
 VecSearchExecutor, Expr parser — compiled unmodified) with VecSearchExecutor::{ctor,Search} and
 ANNGraphSegment::BuildFromVectorTable replaced at link time by integration/epsilla_b200_dropin.cpp, i.e.
-the search and the build run on the B200 through the C ABI while the caller-facing surface is the
+the search and the build run on the GPU through the C ABI while the caller-facing surface is the
 reference's.  Replays the reference's golden tests through that surface."""
 import os
 
@@ -12,13 +12,13 @@ from helpers import assert_same_results, exact_topk, gen, recall
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-DROPIN = os.path.join(ROOT, "integration", "_build", "libepsilla_ref_b200.so")
+DROPIN = os.path.join(ROOT, "oracle", "_ref", "dropin", "libepsilla_ref_b200.so")
 
 
 @pytest.fixture(scope="module")
 def Drop():
     if not os.path.exists(DROPIN):
-        pytest.skip("integration/_build/libepsilla_ref_b200.so was not built (needs /root/reference at build time)")
+        pytest.skip("oracle/_ref/dropin/libepsilla_ref_b200.so was not built (needs a reference checkout at build time)")
     from oracle.oracle import Ref
 
     def make(metric, dim, cap, cols=()):

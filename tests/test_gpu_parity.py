@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box).  Every call goes through the C ABI
+"""GPU parity tests (run with -m gpu on an H100).  Every call goes through the C ABI
 (libepsilla_b200.so via vectordb_b200.Index); the checker is the oracle (oracle_port.c, and the compiled
 reference oracle/_ref/libepsilla_ref.so when it travelled) and the committed golden fixtures."""
 import numpy as np
@@ -260,7 +260,7 @@ def test_device_api_and_shard_merge(vdb):
         ix.close()
 
 
-# ---- exact scan on the tensor cores: coarse tcgen05 pass (tf32 / bf16 mirror) + fp32 re-score -------------------
+# ---- exact scan on the tensor cores: coarse wgmma pass (tf32 / bf16 mirror) + fp32 re-score -------------------
 def test_exact_scan_coarse_modes_match_oracle(vdb, port):
     n, d, nq, k = 60000, 96, 128, 10
     X, Q = gen(n, d, 301), gen(nq, d, 302)
@@ -531,7 +531,7 @@ def test_sharded_search_two_ranks(vdb, tmp_path):
     of the whole table."""
     import torch
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     import torch.multiprocessing as mp
     uid_path, out_path = str(tmp_path / "uid.bin"), str(tmp_path / "out%d.npz")
     mp.spawn(_shard_worker, args=(2, uid_path, out_path), nprocs=2, join=True)
@@ -575,43 +575,38 @@ def test_string_codes_filter_through_c_abi(vdb):
     ix.close()
 
 
-def test_facets_match_reference(vdb, have_ref):
+def test_facets_match_reference(vdb):
     """f4: FacetExecutor::Aggregate on the device (eps_facet_batch) against the reference's own FacetExecutor on the
-    same result lists: int / double / bool / string keys, SUM / COUNT / MIN / MAX, '@distance' inside an aggregate."""
-    if not have_ref:
-        pytest.skip("oracle/_ref/libepsilla_ref.so did not travel")
-    from oracle.oracle import Ref
+    same result lists (fixture facets: the reference's attribute table, parsed expressions and JSON answers): int /
+    double / bool / string keys, SUM / COUNT / MIN / MAX, '@distance' inside an aggregate."""
+    import json
+    import os
+    g = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "facets.npz"), allow_pickle=False)
     n, d, nq, k = 4000, 16, 12, 64
     X, Q = gen(n, d, 111), gen(nq, d, 112)
     rng = np.random.default_rng(113)
-    cols = [("ID", "int4"), ("w", "double"), ("flag", "bool"), ("name", "string")]
-    r = Ref("l2", d, n, cols)
-    r.set_rows(X)
-    idv, wv, fv = np.arange(n), rng.random(n), rng.integers(0, 2, n)
+    rng.random(n), rng.integers(0, 2, n)  # the ID / w / flag columns, already in the fixture's attribute table
     names = ["n%d" % v for v in rng.integers(0, 9, n)]
-    for nm, v in (("ID", idv), ("w", wv), ("flag", fv)):
-        r.set_attr_column(nm, v)
-    r.set_string_column("name", names)
     ix = vdb.Index("l2", d, host_vectors=X)
     ix.sync_rows(n)
-    ix.set_attrs(r.attrs[: n * r.stride].copy(), r.stride, n)
+    ix.set_attrs(g["attrs"], int(g["stride"]), n)
     dictionary = {s: i for i, s in enumerate(sorted(set(names)))}
     back = {i: s for s, i in dictionary.items()}
-    ix.set_string_codes(r.attr_offset("name"), 0, np.array([dictionary[s] for s in names], np.int32))
+    ix.set_string_codes(int(g["name_offset"]), 0, np.array([dictionary[s] for s in names], np.int32))
     ix.config(500, 500, force_brute=True)
-    ids, ds, cnt, _ = ix.search(Q, k)
+    sids, sds, scnt, _ = ix.search(Q, k)
+    assert_same_results(sids, sds, scnt, g["ids"], g["dists"], g["counts"], "facet result lists")
+    ids, ds, cnt = g["ids"], g["dists"].astype(np.float32), g["counts"]   # the lists the reference aggregated
     AGG = {"SUM": 30, "MIN": 31, "MAX": 32, "COUNT": 33}
     cases = [("ID % 7", ["SUM(w)", "COUNT(*)", "MIN(ID)", "MAX(w * 2 + @distance)"]), ("name", ["COUNT(*)", "SUM(ID)"]),
              ("flag", ["COUNT(*)", "MAX(@distance)"]), ("w * 2", ["COUNT(*)"]), ("", ["COUNT(*)", "SUM(w)", "MIN(@distance)"])]
-    for group, aggs in cases:
-        knodes, ktype = r.value_nodes(group if group else "1")
-        alist = []
-        for a in aggs:
-            inner = "1" if a.upper().startswith("COUNT(") else a[a.index("(") + 1:-1]
-            alist.append((AGG[a[:a.index("(")].upper()], r.value_nodes(inner)[0]))
+    for ci, (group, aggs) in enumerate(cases):
+        knodes, ktype = g["key_nodes_%d" % ci], int(g["key_type_%d" % ci])
+        alist = [(AGG[a[:a.index("(")].upper()], g["agg_nodes_%d_%d" % (ci, ai)]) for ai, a in enumerate(aggs)]
         got = ix.facet(ids, cnt, knodes, ktype, alist, dists=ds)
+        want_all = json.loads(str(g["want_%d" % ci]))
         for q in range(nq):
-            want = r.facet(group, aggs, ids[q, :cnt[q]], ds[q, :cnt[q]])
+            want = want_all[q]
             assert len(got[q]) == len(want), (group, q)
             wmap = {}
             for obj in want:

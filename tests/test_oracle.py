@@ -1,12 +1,18 @@
 """CPU tests: the oracle restatement (oracle/oracle_port.c) against the reference's golden vectors
-(tests/golden, generated from the compiled reference) and — where oracle/_ref/libepsilla_ref.so exists —
-against the reference itself, bit for bit."""
+(tests/golden, generated from the compiled reference by tests/golden/make_golden.py), bit for bit."""
+import os
+
 import numpy as np
 import pytest
 
 from helpers import gen
 
 METRICS = ("l2", "ip", "cosine")
+
+
+@pytest.fixture(scope="module")
+def refchecks():
+    return np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "refchecks.npz"), allow_pickle=False)
 
 
 def test_dense_vector_known_answers(port, golden):
@@ -88,66 +94,48 @@ def test_prepare_init_ids(port, golden):
     assert rest[0] == (nav + 1) % 2000 or (nav + 1) % 2000 in row
 
 
-def test_distances_bitexact_vs_reference(port, have_ref):
-    if not have_ref:
-        pytest.skip("oracle/_ref/libepsilla_ref.so not present")
-    from oracle.oracle import Ref
+def test_distances_bitexact_vs_reference(port, refchecks):
     rng = np.random.default_rng(7)
+    want = iter(refchecks["dist"])
     for d in list(range(1, 40)) + [127, 128, 130, 131, 768, 769, 770, 771, 1536]:
-        r = {m: Ref(m, d, 4) for m in METRICS}
         for _ in range(4):
             a, b = rng.standard_normal(d).astype(np.float32), rng.random(d, dtype=np.float32)
-            for m in METRICS:
-                x, y = r[m].distance(a, b), port.distance(m, a, b)
+            for m, x in zip(METRICS, next(want)):
+                y = port.distance(m, a, b)
                 assert np.float32(x).tobytes() == np.float32(y).tobytes(), (d, m, x, y)
     a = rng.random(333, dtype=np.float32)
-    assert np.array_equal(r["l2"].normalize(a), port.normalize(a))
+    assert np.array_equal(refchecks["normalized"], port.normalize(a))
 
 
-def test_port_matches_reference_search_live(port, have_ref):
-    """Fresh seeded table, graph built by the reference here, port vs VecSearchExecutor (T=1)."""
-    if not have_ref:
-        pytest.skip("oracle/_ref/libepsilla_ref.so not present")
-    from oracle.oracle import Ref
+def test_port_matches_reference_search_live(port, refchecks):
+    """Seeded table with the graph the reference built on it (fixture refchecks): port vs VecSearchExecutor (T=1)
+    without filter, with an attribute filter and with a distance filter."""
+    g = refchecks
     n, d = 3000, 24
     X, Q = gen(n, d, 5), gen(12, d, 6)
-    r = Ref("l2", d, n, [("ID", "int4")])
-    r.set_rows(X)
-    r.set_attr_column("ID", np.arange(n))
-    ni, off, nb, nav = r.build(threads=2)
-    r.make_executors(1, 1, 500, counting=True)
-    for f in ("", "ID >= 1500", "@distance > 1.0"):
-        nodes = r.filter_nodes(f)
-        for q in Q:
-            a, b, c = r.search(q, 20, f)
-            ids, ds, cnt, st = port.search_batch(metric="l2", vectors=X, queries=q, limit=20, n_indexed=ni, offsets=off,
-                                                 nbrs=nb, nav=nav, attrs=r.attrs, attr_stride=r.stride,
-                                                 filter_nodes=nodes)
-            assert cnt[0] == len(a) and np.array_equal(ids[0, :len(a)], a) and np.array_equal(ds[0, :len(a)], b)
-            assert st[0] == c
+    graph = dict(n_indexed=int(g["live_n_indexed"]), offsets=g["live_offsets"], nbrs=g["live_nbrs"].astype(np.int64),
+                 nav=int(g["live_nav"]))
+    for fi in range(3):
+        nodes = g["live_nodes_%d" % fi]
+        for qi, q in enumerate(Q):
+            n_want = int(g["live_counts_%d" % fi][qi])
+            a, b = g["live_ids_%d" % fi][qi, :n_want], g["live_dists_%d" % fi][qi, :n_want]
+            ids, ds, cnt, st = port.search_batch(metric="l2", vectors=X, queries=q, limit=20, attrs=g["live_attrs"],
+                                                 attr_stride=int(g["live_stride"]), filter_nodes=nodes, **graph)
+            assert cnt[0] == n_want and np.array_equal(ids[0, :n_want], a) and np.array_equal(ds[0, :n_want], b)
+            assert st[0] == g["live_ndist_%d" % fi][qi]
 
 
-def test_filter_eval_vs_reference(port, have_ref):
-    if not have_ref:
-        pytest.skip("oracle/_ref/libepsilla_ref.so not present")
-    from oracle.oracle import Ref
-    rng = np.random.default_rng(3)
-    n = 64
-    r = Ref("l2", 4, n, [("a", "int1"), ("b", "int2"), ("c", "int4"), ("d", "int8"), ("x", "float"), ("y", "double"),
-                         ("t", "bool")])
-    r.set_rows(rng.random((n, 4), dtype=np.float32))
-    r.set_attr_column("a", rng.integers(-100, 100, n)); r.set_attr_column("b", rng.integers(-1000, 1000, n))
-    r.set_attr_column("c", rng.integers(-10**6, 10**6, n)); r.set_attr_column("d", rng.integers(-10**12, 10**12, n))
-    r.set_attr_column("x", rng.standard_normal(n)); r.set_attr_column("y", rng.standard_normal(n))
-    r.set_attr_column("t", rng.integers(0, 2, n))
-    exprs = ["a < 0", "b >= 10 OR c < 0", "d / 1000 > a * b", "x + y < 0.5", "t = true", "NOT t = false", "t",
-             "NOT (a > 3 AND t = true)", "c % 5 = 2", "@distance < 0.5", "@distance < 0.5 AND a < 1000",
-             "x * @distance > y", "(a + b) * 2 - c / 3 <= d", "a = b OR x <> y", "true", "false OR t"]
-    for e in exprs:
-        nodes = r.filter_nodes(e)
-        for row in range(n):
-            for dist in (0.25, 0.75):
-                assert port.filter_eval(nodes, r.attrs, r.stride, row, dist) == r.filter_eval(e, row, dist), (e, row)
+def test_filter_eval_vs_reference(port, refchecks):
+    """The port's evaluator on the node programs the reference's parser produced (fixture refchecks) against the
+    reference's Expr evaluator on the same typed attribute table: every expression, row and distance."""
+    g = refchecks
+    attrs, stride = g["fe_attrs"], int(g["fe_stride"])
+    for i, e in enumerate(g["fe_exprs"]):
+        nodes = g["fe_nodes_%d" % i]
+        for row in range(attrs.size // stride):
+            for j, dist in enumerate((0.25, 0.75)):
+                assert port.filter_eval(nodes, attrs, stride, row, dist) == g["fe_result"][i, row, j], (e, row)
 
 
 def test_add_into_queue_properties(port):

@@ -3,7 +3,7 @@
   C1  brute-force L2 top-10, 10k x 128, batch = 1 (host-buffer call per query) next to the reference CPU path
   C2  1M x 768 cosine, graph index, batch = 1024, top-10
   C3  10M x 768 L2, graph index, batch = 4096, top-100 + metadata filter (attr = row % 100, "ID < 10", post-filter)
-  C4  10M x 1536 IP, index build + search (batch 1024, top-10)
+  C4  5M x 1536 IP, index build + search (batch 1024, top-10; 31 GB of rows on an 80 GB H100)
   C5  100M x 768 L2 sharded across 8 GPUs (12.5M rows per rank, own graph per shard), batch = 8192, top-10,
       NCCL candidate all-gather inside the library — launch with torchrun --nproc-per-node 8
 
@@ -243,7 +243,7 @@ def main():
         nodes = np.array([[7, 1, -1, -1, 0, 0, 0, 0], [1, 1, -1, -1, 10, 0, 0, -1], [19, 3, 0, 1, 0, 0, 0, -1]], np.int64)  # Int4Attr@0 < 10
         print(json.dumps(graph_config("C3", A.rows or 10_000_000, 768, "l2", 4096, 100, filt=("ID < 10", nodes, 100))))
     elif which == "c4":
-        print(json.dumps(graph_config("C4", A.rows or 10_000_000, 1536, "ip", 1024, 10)))
+        print(json.dumps(graph_config("C4", A.rows or 5_000_000, 1536, "ip", 1024, 10)))
     else:
         import torch.distributed as dist
         from vectordb_b200.sharded import ShardGroup

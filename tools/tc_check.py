@@ -1,4 +1,4 @@
-"""Developer tool: exact-scan results with the tcgen05 coarse pass vs the fp32 SIMT path (EPS_NO_TC=1), same data."""
+"""Developer tool: exact-scan results with the wgmma coarse pass vs the fp32 SIMT path (EPS_NO_TC=1), same data."""
 import os, sys, subprocess, json, time
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,4 +1,4 @@
-"""vectordb_b200 — B200-native (sm_100a) vector-search hot path of Epsilla behind a C ABI.
+"""vectordb_b200 — H100-native (sm_90a) vector-search hot path of Epsilla behind a C ABI.
 
 The product is ``libepsilla_b200.so`` (hand-written CUDA, ``csrc/``) declared in
 ``include/epsilla_b200.h``.  This package is the thin Python host layer used by the tests and

@@ -1,4 +1,4 @@
-// mbarrier / TMA (bulk async copy) primitives shared by the sm_100a kernels of libepsilla_b200
+// mbarrier / TMA (bulk async copy) primitives shared by the sm_90a kernels of libepsilla_b200
 // (tc_dist.cu: 2-D tensor-map loads of operand tiles; graph_search.cu: 1-D bulk copies of gathered rows).
 #pragma once
 #include <cuda_runtime.h>

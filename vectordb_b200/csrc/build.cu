@@ -10,7 +10,8 @@
 //         connectivity repair from the navigation point (CheckConnectivity :687-775);
 //   B3  flatten to the int64 CSR.
 // The reference build is not reproducible (rand(), racy OpenMP), so parity for the build is graph QUALITY
-// (recall / distance evaluations of searches on it), not edge identity (SURVEY.md §8c).
+// (recall / distance evaluations of searches on it), not edge identity (SURVEY.md §8c).  This build is reproducible:
+// seeded choices, fixed-order sums, order-independent reverse lists (tile.cuh rev_push) and list updates.
 //
 // Device mapping:
 //   * kNN lists: exact all-pairs tiles (brute_force.cu) when n <= exact_knn_below, NN-descent local joins
@@ -122,21 +123,21 @@ __global__ void fill_cand_from_knn_kernel(const unsigned long long* __restrict__
   cand[i] = id;
 }
 
-// reverse candidates: for edge v -> p append v to rev[p] (first rev_cap arrivals)
+// reverse candidates: for edge v -> p push v to rev[p] (rev_cap of them, chosen independently of arrival order)
 __global__ void append_reverse_kernel(const int32_t* __restrict__ ids, const int32_t* __restrict__ cnt, int stride,
-                                      int64_t n, int rev_cap, int32_t* __restrict__ rev, int32_t* __restrict__ rev_cnt) {
+                                      int64_t n, int rev_cap, unsigned long long* __restrict__ rev, int32_t* __restrict__ rev_cnt,
+                                      uint32_t salt) {
   const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   const int64_t v = i / stride;
   const int j = static_cast<int>(i % stride);
   if (v >= n || j >= cnt[v]) return;
   const int p = ids[v * stride + j];
-  const int slot = atomicAdd(&rev_cnt[p], 1);
-  if (slot < rev_cap) rev[static_cast<int64_t>(p) * rev_cap + slot] = static_cast<int32_t>(v);
+  rev_push(rev, rev_cap, rev_cnt, p, static_cast<int32_t>(v), salt);
 }
 
 // cand row for pass 2: [v, own list..., reverse candidates not already present...]
 __global__ void fill_cand_union_kernel(const int32_t* __restrict__ ids, const int32_t* __restrict__ cnt, int stride,
-                                       const int32_t* __restrict__ rev, const int32_t* __restrict__ rev_cnt, int rev_cap,
+                                       const unsigned long long* __restrict__ rev, const int32_t* __restrict__ rev_cnt, int rev_cap,
                                        int64_t v0, int batch, int32_t* __restrict__ cand) {
   const int64_t z = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (z >= batch) return;
@@ -148,7 +149,7 @@ __global__ void fill_cand_union_kernel(const int32_t* __restrict__ ids, const in
   for (int j = 0; j < own && m < kC; ++j) c[m++] = ids[v * stride + j];
   const int nr = min(rev_cnt[v], rev_cap);
   for (int j = 0; j < nr && m < kC; ++j) {
-    const int32_t u = rev[v * rev_cap + j];
+    const int32_t u = rev_id(rev[v * rev_cap + j]);
     bool dup = (u == v);
     for (int t = 1; t <= own && !dup; ++t) dup = (c[t] == u);
     if (!dup) c[m++] = u;
@@ -156,23 +157,27 @@ __global__ void fill_cand_union_kernel(const int32_t* __restrict__ ids, const in
   for (; m < kC; ++m) c[m] = -1;
 }
 
-__global__ void column_sum_kernel(const float* __restrict__ vectors, int64_t n, int dim, float* __restrict__ out) {
-  // grid.x covers columns, grid.y splits rows; atomics combine (fp32 sums like nsg.cpp:110-117)
+__global__ void column_sum_kernel(const float* __restrict__ vectors, int64_t n, int dim, float* __restrict__ part) {
+  // grid.x covers columns, grid.y splits rows into slices; part[slice * dim + col] (fp32 sums like nsg.cpp:110-117)
   const int col = blockIdx.x * blockDim.x + threadIdx.x;
   if (col >= dim) return;
   const int64_t per = (n + gridDim.y - 1) / gridDim.y;
   const int64_t r0 = blockIdx.y * per, r1 = min(n, r0 + per);
   float s = 0.f;
   for (int64_t r = r0; r < r1; ++r) s += vectors[r * dim + col];
-  atomicAdd(&out[col], s);
+  part[static_cast<int64_t>(blockIdx.y) * dim + col] = s;
 }
-__global__ void scale_kernel(float* v, int n, float s) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) v[i] *= s;
+// centroid = the slices' sums added in slice order (a fixed order: the navigation point is reproducible) / n
+__global__ void centroid_kernel(const float* __restrict__ part, int slices, int dim, float inv_n, float* __restrict__ out) {
+  const int col = blockIdx.x * blockDim.x + threadIdx.x;
+  if (col >= dim) return;
+  float s = 0.f;
+  for (int y = 0; y < slices; ++y) s += part[static_cast<int64_t>(y) * dim + col];
+  out[col] = s * inv_n;
 }
 
 static int prune_pass(Index* ix, int64_t n, const unsigned long long* d_knn, int K, bool pass2, int out_degree,
-                      int pool_cap, int min_degree, float alpha, int32_t* d_ids, float* d_dist, int32_t* d_cnt, int stride, const int32_t* d_rev,
+                      int pool_cap, int min_degree, float alpha, int32_t* d_ids, float* d_dist, int32_t* d_cnt, int stride, const unsigned long long* d_rev,
                       const int32_t* d_rev_cnt, int rev_cap, int32_t* d_ids_out, float* d_dist_out, int32_t* d_cnt_out,
                       eps_stats* st) {
   const int64_t batch_max = 4096;
@@ -263,13 +268,15 @@ int build_graph(Index* ix, int64_t n, const eps_build_params* params) {
   // ---- B2a: navigation point = exact nearest row to the centroid (L2) ----------------------
   int64_t nav = 0;
   {
-    DevBuf cen, top;
+    DevBuf cen, part, top;
+    const unsigned slices = static_cast<unsigned>(std::min<int64_t>(1024, (n + 255) / 256));
     EPS_TRY(cen.reserve(static_cast<size_t>(ix->dim) * 4));
+    EPS_TRY(part.reserve(static_cast<size_t>(ix->dim) * slices * 4));
     EPS_TRY(top.reserve(8));
-    EPS_CUDA(cudaMemsetAsync(cen.p, 0, static_cast<size_t>(ix->dim) * 4, ix->stream));
-    dim3 g(static_cast<unsigned>((ix->dim + 127) / 128), static_cast<unsigned>(std::min<int64_t>(1024, (n + 255) / 256)));
-    column_sum_kernel<<<g, 128, 0, ix->stream>>>(ix->d_vectors, n, static_cast<int>(ix->dim), cen.as<float>());
-    scale_kernel<<<static_cast<unsigned>((ix->dim + 127) / 128), 128, 0, ix->stream>>>(cen.as<float>(), static_cast<int>(ix->dim), 1.0f / static_cast<float>(n));
+    dim3 g(static_cast<unsigned>((ix->dim + 127) / 128), slices);
+    column_sum_kernel<<<g, 128, 0, ix->stream>>>(ix->d_vectors, n, static_cast<int>(ix->dim), part.as<float>());
+    centroid_kernel<<<static_cast<unsigned>((ix->dim + 127) / 128), 128, 0, ix->stream>>>(
+        part.as<float>(), static_cast<int>(slices), static_cast<int>(ix->dim), 1.0f / static_cast<float>(n), cen.as<float>());
     const int saved_metric = ix->metric;
     const bool saved_del = ix->any_deleted;
     ix->metric = EPS_METRIC_L2;
@@ -283,6 +290,7 @@ int build_graph(Index* ix, int64_t n, const eps_build_params* params) {
     EPS_CUDA(cudaStreamSynchronize(ix->stream));
     nav = key_id(key);
     cen.release();
+    part.release();
     top.release();
   }
 
@@ -297,20 +305,22 @@ int build_graph(Index* ix, int64_t n, const eps_build_params* params) {
 
   // ---- B2c: reverse edges (InterInsert) ----------------------------------------------------
   const int rev_cap = kC - 1 - R;  // union always fits the candidate slots
-  EPS_TRY(rev.reserve(static_cast<size_t>(n) * rev_cap * 4));
+  EPS_TRY(rev.reserve(static_cast<size_t>(n) * rev_cap * 8));
   EPS_TRY(rev_cnt.reserve(static_cast<size_t>(n) * 4));
+  EPS_CUDA(cudaMemsetAsync(rev.p, 0xFF, static_cast<size_t>(n) * rev_cap * 8, ix->stream));
   EPS_CUDA(cudaMemsetAsync(rev_cnt.p, 0, static_cast<size_t>(n) * 4, ix->stream));
   {
     const int64_t tot = n * stride;
     append_reverse_kernel<<<static_cast<unsigned>((tot + 255) / 256), 256, 0, ix->stream>>>(
-        ids1.as<int32_t>(), cnt1.as<int32_t>(), stride, n, rev_cap, rev.as<int32_t>(), rev_cnt.as<int32_t>());
+        ids1.as<int32_t>(), cnt1.as<int32_t>(), stride, n, rev_cap, rev.as<unsigned long long>(), rev_cnt.as<int32_t>(),
+        0x68E31DA4u + static_cast<uint32_t>(bp.seed));
     EPS_CUDA(cudaGetLastError());
   }
   EPS_TRY(ids2.reserve(static_cast<size_t>(n) * stride * 4));
   EPS_TRY(dist2.reserve(static_cast<size_t>(n) * stride * 4));
   EPS_TRY(cnt2.reserve(static_cast<size_t>(n) * 4));
   EPS_TRY(prune_pass(ix, n, nullptr, 0, true, R, kC, min_deg, alpha, ids1.as<int32_t>(), dist1.as<float>(), cnt1.as<int32_t>(), stride,
-                     rev.as<int32_t>(), rev_cnt.as<int32_t>(), rev_cap, ids2.as<int32_t>(), dist2.as<float>(),
+                     rev.as<unsigned long long>(), rev_cnt.as<int32_t>(), rev_cap, ids2.as<int32_t>(), dist2.as<float>(),
                      cnt2.as<int32_t>(), &st));
 
   // ---- B2d + B3: connectivity repair and CSR flatten (host, integer work) -------------------

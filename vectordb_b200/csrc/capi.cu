@@ -255,7 +255,7 @@ using eps::Index;
 extern "C" {
 
 const char* eps_last_error(void) { return eps::g_err.c_str(); }
-const char* eps_version(void) { return "epsilla_b200 0.1 (sm_100a)"; }
+const char* eps_version(void) { return "epsilla_b200 0.1 (sm_90a)"; }
 int eps_device_count(void) {
   int n = 0;
   if (cudaGetDeviceCount(&n) != cudaSuccess) return 0;

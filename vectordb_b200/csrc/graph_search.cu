@@ -26,16 +26,16 @@
 //     occupied slots, evaluates up to 8 landed rows with all 32 lanes on every row (float4 from shared memory, the
 //     lane's query chunk loaded once, 5 shuffle steps per row), refills its slots from the FIFO and keeps streaming
 //     while the FIFO has a backlog; accepted keys (key < worst-in-queue) go to a small pending buffer that is merged
-//     into the sorted queue by a block-parallel rank-and-shift when it fills (or after every expansion in exact mode);
+//     into the sorted queue by a block-parallel rank-and-shift, at the latest when the expansion is consumed;
 //   * adjacency: fixed-stride rows of 64 int32 ids (one 256-byte read from the vertex id; longer rows
 //     continue in the CSR); visited: one bitmap per in-flight query in global memory, atomicOr test-and-set,
 //     cleared by the CTA after the query like the reference clears its vector<bool> (:711-714) — on large tables
 //     only the words the query touched, from a log of its fresh ids.
-// exact mode (search width 1): one candidate per iteration, rows consumed and merged before the next pick —
-//   the visit order, results and distance-evaluation counts of the reference at IntraQueryThreads = 1.
-// wide mode (width W = 2..8): up to W candidates are picked per iteration from queue ∪ pending while the rows
-//   of the previous iteration are still in flight — the device analogue of IntraQueryThreads > 1; like that
-//   mode it is not bit-identical to the sequential order.
+// every iteration picks up to W (the search width) unchecked candidates, and the next pick waits until all their rows
+//   are consumed and merged.  Width 1 has the visit order, results and distance-evaluation counts of the reference
+//   at IntraQueryThreads = 1; widths 2..8 expand W candidates together — the device analogue of IntraQueryThreads > 1,
+//   not bit-identical to the sequential order but, unlike that racy mode, the same on every run: the queue after a
+//   merge is the best L of the queue and all fresh rows, whatever order the rows land in.
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -82,8 +82,7 @@ struct GSArgs {
   int dim, metric, vec4;
   int L, Lp;
   int nq;
-  int W;                          // candidates per iteration (1 in exact mode)
-  int exact;
+  int W;                          // candidates per iteration (the search width)
   int R;                          // ring slots (slot s is owned by consumer warp s % 3)
   int fc;                         // fresh-id FIFO capacity (power of two)
   unsigned long long* qtimes;     // developer build: [nq x 2] globaltimer at query start / end (null otherwise)
@@ -330,8 +329,8 @@ __global__ void __launch_bounds__(kGsThreads, 7) graph_search_kernel(GSArgs a) {
       const int m = s_npend;
       const uint32_t head = s_head;
       const int ncont = s_ncont;
-      // -- D: merge the pending keys (every time in exact mode; when the buffer could overflow otherwise) --
-      const bool merged = m > 0 && (a.exact || m > kPC - R);
+      // -- D: merge the pending keys --
+      const bool merged = m > 0;
       // s_npend / s_head are bumped by the consumer phase below: no thread may get there before EVERY thread has taken
       // the snapshot above (the merge's own barriers do that when there is a merge)
       if (merged) merge_pending(qa, pend, cs, pos, m, L, &s_npend, &s_cursor, ubits);
@@ -339,9 +338,8 @@ __global__ void __launch_bounds__(kGsThreads, 7) graph_search_kernel(GSArgs a) {
       GS_T(tm1);
       GS_ACC(1, tx1, tm1);
       const bool idle = inflight == 0 && head == fifo_tail;
-      // A runs when the ring cannot be kept full from the backlog alone (wide) / when the previous expansion
-      // has been consumed and merged (exact)
-      const bool want = a.exact ? idle : (fifo_tail - head) < static_cast<uint32_t>(R);
+      // A runs when the previous expansion has been consumed and merged
+      const bool want = idle;
 
       // -- C/B, per consumer warp: distances of the landed rows of its slots, then refill every slot from the FIFO.
       // The warp keeps streaming (consume, refill, consume ...) without coming back to the block barrier while the FIFO
@@ -765,7 +763,7 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   a.stats = ix->s_misc.as<unsigned long long>();
   a.visited_words = words; a.seed_ld = seed_ld; a.dim = dim; a.metric = ix->metric;
   a.vec4 = ix->vec4 ? 1 : 0; a.L = static_cast<int>(L); a.Lp = Lp; a.nq = static_cast<int>(nq);
-  a.W = width; a.exact = width == 1 ? 1 : 0; a.R = R; a.slot_bytes = slot_bytes; a.fc = fc;
+  a.W = width; a.R = R; a.slot_bytes = slot_bytes; a.fc = fc;
   a.qtimes = nullptr;
 #ifdef EPS_GS_PROFILE
   EPS_TRY(ix->s_tail.reserve(static_cast<size_t>(nq) * 32));  // borrowed scratch (the hybrid tail buffer is filled after the search)

@@ -79,12 +79,12 @@ struct Index {
 
   cudaStream_t stream = nullptr;
   cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-  int num_sms = 148;
+  int num_sms = 132;
 
   // scratch
   DevBuf s_queries, s_dist, s_topk, s_topk2, s_pass, s_filter, s_visited, s_vlog, s_queue, s_tail, s_out_ids, s_out_dists,
       s_out_counts, s_stats, s_misc, s_seed_rows, s_seed_dist, s_xnorm, s_qnorm, s_coarse, s_thr, s_cand, s_cand_cnt, s_bf16, s_qbf16, s_flags;
-  int coarse_mode = 1;           // exact-scan coarse pass: 0 = fp32 SIMT only, 1 = tcgen05 TF32, 2 = tcgen05 bf16 mirror
+  int coarse_mode = 1;           // exact-scan coarse pass: 0 = fp32 SIMT only, 1 = wgmma TF32, 2 = wgmma bf16 mirror
   int coarse_guard = 1;          // verify the coarse pass after the re-score and redo unsafe queries (brute_force.cu)
   int coarse_boost = 1;          // multiplier of k' learnt by the guard for this table (1, 4, 16, 64)
   int64_t bf16_rows = 0;
@@ -114,7 +114,7 @@ int brute_force_topk(Index* ix, const float* d_queries, int64_t nq, int64_t row_
 int launch_distances(Index* ix, const float* A_base, int64_t row_start, int64_t n, const float* d_queries, int64_t nq,
                      float* D, int64_t ldd, uint64_t* launches);
 
-// tc_dist.cu: tcgen05 TF32 coarse distances (same contract as launch_distances, values carry ~1e-3 rel. error)
+// tc_dist.cu: wgmma TF32 / BF16 coarse distances (same contract as launch_distances, values carry ~1e-3 rel. error)
 bool tc_dist_usable(const Index* ix, int64_t nq);
 struct TcFused {             // fused threshold selection in the epilogue (no distance tile written)
   const float* thr;          // [nq] running coarse k'-th best

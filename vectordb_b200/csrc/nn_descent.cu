@@ -14,8 +14,10 @@
 //   * updates are selective (the two closest join partners of every candidate), applied by a warp under a
 //     per-list spin lock with a coalesced load / ballot-rank / shuffle-shift / store of the sorted list;
 //   * sampling, reverse lists and flags are integer passes over the lists.
-// Like the reference (rand(), random_shuffle, racy OpenMP) the result is not bit-reproducible; parity is
-// graph quality (SURVEY.md §8c).
+// Unlike the reference (rand(), random_shuffle, racy OpenMP) the result is reproducible: the initial lists are seeded,
+// a list after a local-join launch is the best K of its old entries and every proposal whatever the insertion order,
+// reverse lists keep a hash-chosen subset (rev_push), and the convergence test counts the entries a list gained over
+// the iteration rather than racy insert successes.  Parity with the reference is graph quality (SURVEY.md §8c).
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -26,11 +28,6 @@
 namespace eps {
 
 constexpr int kHalf = kC / 2;  // 64 new + 64 old slots
-
-__device__ __forceinline__ uint32_t mix32(uint32_t x) {
-  x ^= x >> 16; x *= 0x7feb352dU; x ^= x >> 15; x *= 0x846ca68bU; x ^= x >> 16;
-  return x;
-}
 
 // Random initial lists (nndescent.hpp:76-91): K pseudo-random ids per vertex, distances evaluated, sorted,
 // duplicates blanked.  One CTA (128 threads) per vertex.  All entries start "new" (flag bit clear).
@@ -64,15 +61,17 @@ __global__ void __launch_bounds__(128) nnd_init_kernel(const float* __restrict__
 
 // Sampling (nndescent.hpp:139-170): up to S new entries (closest first) become this iteration's nn_new and
 // lose their flag; up to S old entries become nn_old.  Also appends the vertex to the reverse lists of the
-// sampled neighbours (:173-180), first-come up to S each.  One thread per vertex.
-__global__ void nnd_sample_kernel(unsigned long long* __restrict__ knn, int64_t n, int K, int S,
-                                  int32_t* __restrict__ fnew, int32_t* __restrict__ fold, int32_t* __restrict__ rnew,
-                                  int32_t* __restrict__ rold, int32_t* __restrict__ rnew_cnt,
-                                  int32_t* __restrict__ rold_cnt) {
+// sampled neighbours (:173-180), up to S each (rev_push).  Snapshots the ids of the list for the convergence
+// count.  One thread per vertex.
+__global__ void nnd_sample_kernel(unsigned long long* __restrict__ knn, int64_t n, int K, int S, uint32_t salt,
+                                  int32_t* __restrict__ fnew, int32_t* __restrict__ fold, unsigned long long* __restrict__ rnew,
+                                  unsigned long long* __restrict__ rold, int32_t* __restrict__ rnew_cnt,
+                                  int32_t* __restrict__ rold_cnt, int32_t* __restrict__ snap) {
   const int64_t v = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (v >= n) return;
   unsigned long long* list = knn + v * K;
   int nn = 0, no = 0;
+  for (int j = 0; j < K; ++j) snap[v * K + j] = (list[j] & kKeyMask) == kKeyInf ? -1 : static_cast<int32_t>(key_id(list[j]));
   for (int j = 0; j < K; ++j) {
     const unsigned long long key = list[j];
     if ((key & kKeyMask) == kKeyInf) break;
@@ -81,13 +80,11 @@ __global__ void nnd_sample_kernel(unsigned long long* __restrict__ knn, int64_t 
       if (nn < S) {
         fnew[v * S + nn++] = u;
         list[j] = key | kCheckedBit;
-        const int slot = atomicAdd(&rnew_cnt[u], 1);
-        if (slot < S) rnew[static_cast<int64_t>(u) * S + slot] = static_cast<int32_t>(v);
+        rev_push(rnew, S, rnew_cnt, u, static_cast<int32_t>(v), salt);
       }
     } else if (no < S) {
       fold[v * S + no++] = u;
-      const int slot = atomicAdd(&rold_cnt[u], 1);
-      if (slot < S) rold[static_cast<int64_t>(u) * S + slot] = static_cast<int32_t>(v);
+      rev_push(rold, S, rold_cnt, u, static_cast<int32_t>(v), salt ^ 0x5bd1e995u);
     }
   }
   for (; nn < S; ++nn) fnew[v * S + nn] = -1;
@@ -97,7 +94,7 @@ __global__ void nnd_sample_kernel(unsigned long long* __restrict__ knn, int64_t 
 // Candidate rows of a batch of vertices: [new fwd | new rev | old fwd | old rev], duplicates blanked.
 // One warp per vertex.
 __global__ void nnd_fill_cand_kernel(const int32_t* __restrict__ fnew, const int32_t* __restrict__ fold,
-                                     const int32_t* __restrict__ rnew, const int32_t* __restrict__ rold,
+                                     const unsigned long long* __restrict__ rnew, const unsigned long long* __restrict__ rold,
                                      const int32_t* __restrict__ rnew_cnt, const int32_t* __restrict__ rold_cnt, int S,
                                      int64_t v0, int batch, int32_t* __restrict__ cand) {
   const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
@@ -109,11 +106,11 @@ __global__ void nnd_fill_cand_kernel(const int32_t* __restrict__ fnew, const int
     int32_t id = -1;
     if (s < kHalf) {
       if (s < S) id = fnew[v * S + s];
-      else if (s - S < nrn && s - S < kHalf - S) id = rnew[v * S + (s - S)];
+      else if (s - S < nrn && s - S < kHalf - S) id = rev_id(rnew[v * S + (s - S)]);
     } else {
       const int t = s - kHalf;
       if (t < S) id = fold[v * S + t];
-      else if (t - S < nro && t - S < kHalf - S) id = rold[v * S + (t - S)];
+      else if (t - S < nro && t - S < kHalf - S) id = rev_id(rold[v * S + (t - S)]);
     }
     if (id == v) id = -1;
     c[s] = id;
@@ -187,16 +184,15 @@ __device__ int nnd_insert(unsigned long long* __restrict__ knn, int* __restrict_
 // partners.  One CTA of 128 threads per vertex; thread i scans row i, then the 4 warps apply the proposals.
 __global__ void __launch_bounds__(128) nnd_join_kernel(const int32_t* __restrict__ cand, const float* __restrict__ D,
                                                       int batch, int K, unsigned long long* __restrict__ knn,
-                                                      int* __restrict__ locks, unsigned long long* __restrict__ n_updates) {
+                                                      int* __restrict__ locks) {
   __shared__ int ids[kC];
   __shared__ int p_target[2 * kC];
   __shared__ unsigned long long p_key[2 * kC];
   __shared__ int n_prop;
-  __shared__ int n_done;
   const int z = blockIdx.x;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   ids[tid] = cand[static_cast<int64_t>(z) * kC + tid];
-  if (tid == 0) { n_prop = 0; n_done = 0; }
+  if (tid == 0) n_prop = 0;
   __syncthreads();
   const int me = ids[tid];
   if (me >= 0) {
@@ -217,11 +213,32 @@ __global__ void __launch_bounds__(128) nnd_join_kernel(const int32_t* __restrict
   }
   __syncthreads();
   const int np = n_prop;
-  int mine = 0;
-  for (int p = warp; p < np; p += 4) mine += nnd_insert(knn, locks, K, p_target[p], p_key[p], lane);
-  if (lane == 0 && mine) atomicAdd(&n_done, mine);
-  __syncthreads();
-  if (tid == 0 && n_done) atomicAdd(n_updates, static_cast<unsigned long long>(n_done));
+  for (int p = warp; p < np; p += 4) nnd_insert(knn, locks, K, p_target[p], p_key[p], lane);
+}
+
+// Updates of an iteration (knn.hpp:104-108): entries of the lists that were not in them when it was sampled.  One warp
+// per vertex, K <= 128.
+__global__ void nnd_count_updates_kernel(const unsigned long long* __restrict__ knn, const int32_t* __restrict__ snap,
+                                         int64_t n, int K, unsigned long long* __restrict__ n_updates) {
+  const int64_t v = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (v >= n) return;
+  int32_t f[4];
+  bool seen[4] = {false, false, false, false};
+  for (int h = 0; h < 4; ++h) {
+    const int e = lane + 32 * h;
+    const unsigned long long key = e < K ? knn[v * K + e] : kKeyInf;
+    f[h] = (key & kKeyMask) == kKeyInf ? -1 : static_cast<int32_t>(key_id(key));
+  }
+  for (int t = 0; t < K; ++t) {
+    const int32_t s = snap[v * K + t];
+#pragma unroll
+    for (int h = 0; h < 4; ++h) seen[h] |= f[h] == s;
+  }
+  int fresh = 0;
+#pragma unroll
+  for (int h = 0; h < 4; ++h) fresh += __popc(__ballot_sync(kFull, f[h] >= 0 && !seen[h]));
+  if (lane == 0 && fresh) atomicAdd(n_updates, static_cast<unsigned long long>(fresh));
 }
 
 __global__ void nnd_clear_flags_kernel(unsigned long long* knn, int64_t total) {
@@ -241,11 +258,12 @@ int nn_descent(Index* ix, int64_t n, int K, const eps_build_params& bp, unsigned
                                                                            ix->vec4 ? 1 : 0, K, 0x1234567u + bp.seed, d_knn);
   EPS_CUDA(cudaGetLastError());
 
-  DevBuf fnew, fold, rnew, rold, rnc, roc, locks, cand, D, counter;
+  DevBuf fnew, fold, rnew, rold, rnc, roc, locks, cand, D, counter, snap;
   EPS_TRY(fnew.reserve(static_cast<size_t>(n) * S * 4));
   EPS_TRY(fold.reserve(static_cast<size_t>(n) * S * 4));
-  EPS_TRY(rnew.reserve(static_cast<size_t>(n) * S * 4));
-  EPS_TRY(rold.reserve(static_cast<size_t>(n) * S * 4));
+  EPS_TRY(rnew.reserve(static_cast<size_t>(n) * S * 8));
+  EPS_TRY(rold.reserve(static_cast<size_t>(n) * S * 8));
+  EPS_TRY(snap.reserve(static_cast<size_t>(n) * K * 4));
   EPS_TRY(rnc.reserve(static_cast<size_t>(n) * 4));
   EPS_TRY(roc.reserve(static_cast<size_t>(n) * 4));
   EPS_TRY(locks.reserve(static_cast<size_t>(n) * 4));
@@ -260,19 +278,24 @@ int nn_descent(Index* ix, int64_t n, int K, const eps_build_params& bp, unsigned
     EPS_CUDA(cudaMemsetAsync(rnc.p, 0, static_cast<size_t>(n) * 4, ix->stream));
     EPS_CUDA(cudaMemsetAsync(roc.p, 0, static_cast<size_t>(n) * 4, ix->stream));
     EPS_CUDA(cudaMemsetAsync(counter.p, 0, 8, ix->stream));
+    EPS_CUDA(cudaMemsetAsync(rnew.p, 0xFF, static_cast<size_t>(n) * S * 8, ix->stream));
+    EPS_CUDA(cudaMemsetAsync(rold.p, 0xFF, static_cast<size_t>(n) * S * 8, ix->stream));
     nnd_sample_kernel<<<static_cast<unsigned>((n + 127) / 128), 128, 0, ix->stream>>>(
-        d_knn, n, K, S, fnew.as<int32_t>(), fold.as<int32_t>(), rnew.as<int32_t>(), rold.as<int32_t>(), rnc.as<int32_t>(),
-        roc.as<int32_t>());
+        d_knn, n, K, S, 0x2545F491u * static_cast<uint32_t>(it + 1) + static_cast<uint32_t>(bp.seed), fnew.as<int32_t>(),
+        fold.as<int32_t>(), rnew.as<unsigned long long>(), rold.as<unsigned long long>(), rnc.as<int32_t>(), roc.as<int32_t>(),
+        snap.as<int32_t>());
     for (int64_t v0 = 0; v0 < n; v0 += batch_max) {
       const int batch = static_cast<int>(std::min(batch_max, n - v0));
       nnd_fill_cand_kernel<<<(batch * 32 + 127) / 128, 128, 0, ix->stream>>>(
-          fnew.as<int32_t>(), fold.as<int32_t>(), rnew.as<int32_t>(), rold.as<int32_t>(), rnc.as<int32_t>(), roc.as<int32_t>(),
+          fnew.as<int32_t>(), fold.as<int32_t>(), rnew.as<unsigned long long>(), rold.as<unsigned long long>(), rnc.as<int32_t>(),
+          roc.as<int32_t>(),
           S, v0, batch, cand.as<int32_t>());
       EPS_TRY(launch_pair_tiles(ix, ix->metric, cand.as<int32_t>(), D.as<float>(), batch));
-      nnd_join_kernel<<<batch, 128, 0, ix->stream>>>(cand.as<int32_t>(), D.as<float>(), batch, K, d_knn, locks.as<int>(),
-                                                     counter.as<unsigned long long>());
+      nnd_join_kernel<<<batch, 128, 0, ix->stream>>>(cand.as<int32_t>(), D.as<float>(), batch, K, d_knn, locks.as<int>());
       if (st) st->kernel_launches += 3;
     }
+    nnd_count_updates_kernel<<<static_cast<unsigned>((n * 32 + 255) / 256), 256, 0, ix->stream>>>(
+        d_knn, snap.as<int32_t>(), n, K, counter.as<unsigned long long>());
     EPS_CUDA(cudaGetLastError());
     unsigned long long upd = 0;
     EPS_CUDA(cudaMemcpyAsync(&upd, counter.p, 8, cudaMemcpyDeviceToHost, ix->stream));
@@ -286,7 +309,7 @@ int nn_descent(Index* ix, int64_t n, int K, const eps_build_params& bp, unsigned
   nnd_clear_flags_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, ix->stream>>>(d_knn, total);
   EPS_CUDA(cudaStreamSynchronize(ix->stream));
   fnew.release(); fold.release(); rnew.release(); rold.release(); rnc.release(); roc.release();
-  locks.release(); cand.release(); D.release(); counter.release();
+  locks.release(); cand.release(); D.release(); counter.release(); snap.release();
   (void)iters_done;
   return EPS_OK;
 }

@@ -1,17 +1,19 @@
-// K1-TC — coarse distance tiles of the exact scan on the 5th-generation tensor cores (tcgen05, sm_100a).
+// K1-TC — coarse distance tiles of the exact scan on the Hopper tensor cores (wgmma, sm_90a).
 //
 // The large-batch exact scan (BruteForceSearch / PreFilter branch, engine/db/execution/vec_search_executor.cpp
 // :717-831, at batch B) is a dense contraction D[q,r] = <Q[q,:], X[r,:]> with 2*B*N*d flops against N*d*4 bytes
-// (512 flop/B at B = 1024): the fp32 SIMT tile kernel in brute_force.cu sits at 75 % of the SIMT issue rate and
-// still needs 583 ms per 10M x 768 x 1024 batch.  This kernel produces the same [B x chunk] distance tile with
-// tcgen05.mma kind::tf32:
+// (512 flop/B at B = 1024), far more arithmetic per byte than the fp32 SIMT tile kernel in brute_force.cu can
+// issue.  This kernel produces the same [B x chunk] distance tile with warpgroup MMAs (wgmma, TF32 or BF16 inputs,
+// fp32 accumulate):
 //   * operands stay the reference's fp32 rows — TMA (cp.async.bulk.tensor, 128-byte swizzle) stages 128-row x 32-
 //     float blocks of the table and 256-query x 32-float blocks of the query batch into a 4-stage shared-memory
-//     ring; the tensor core reads them as TF32 (no converted copy of the table is kept);
-//   * one elected thread issues 4 MMAs (M128 x N256 x K8) per block into a TMEM accumulator (256 columns, two
-//     accumulators = all 512 columns, so the epilogue of tile t overlaps the MMAs of tile t+1);
-//   * the epilogue warps read TMEM with tcgen05.ld, turn dot products into the metric
-//     (|x|^2 + |q|^2 - 2 dot | 1 - dot | -dot), and store the tile query-major, coalesced.
+//     ring; the tensor cores read them as TF32 (no converted copy of the table is kept);
+//   * warpgroup 0 is the producer (one thread issues the TMA loads); warpgroups 1 and 2 each own 64 rows of the
+//     128-row tile and issue 4 wgmma m64n256k8 per 128-byte block straight from shared-memory descriptors into a
+//     64 x 256 fp32 register accumulator (128 registers per thread), releasing each stage as its MMAs retire;
+//   * the consumer warpgroups turn dot products into the metric in registers (|x|^2 + |q|^2 - 2 dot | 1 - dot |
+//     -dot) and store the tile query-major, or filter it against the running thresholds; meanwhile the producer
+//     keeps filling the ring for the next tile.
 // TF32 products carry ~1e-3 relative error, so this is a COARSE pass: bf_select_kernel keeps k' > k candidates
 // per query and rescore_kernel re-evaluates them with the exact fp32 direct form before the final (distance,id)
 // sort — returned ids/distances are those of the fp32 path (SURVEY.md §7 step 3: "TF32 MMA with fp32 re-score of
@@ -26,17 +28,19 @@
 
 namespace eps {
 
-constexpr int kTcBM = 128;      // table rows per tile  (UMMA M)
-constexpr int kTcBN = 256;      // queries per tile     (UMMA N)
+constexpr int kTcBM = 128;      // table rows per tile  (two consumer warpgroups x wgmma M = 64)
+constexpr int kTcBN = 256;      // queries per tile     (wgmma N)
 constexpr int kTcBK = 32;       // floats per k-block = one 128-byte swizzle atom
 constexpr int kTcStages = 4;
 constexpr int kTcABytes = kTcBM * kTcBK * 4;   // 16 KB
 constexpr int kTcBBytes = kTcBN * kTcBK * 4;   // 32 KB
 constexpr int kTcStageBytes = kTcABytes + kTcBBytes;
-constexpr int kTcThreads = 192;  // warp 0 TMA, warp 1 MMA (+TMEM alloc), warps 2-5 epilogue
-constexpr int kTcStgCap = 512;   // staged survivors per epilogue warp (8-byte key + 2-byte query index each)
-constexpr int kTcStgBytes = 4 * kTcStgCap * 10 + 16;
+constexpr int kTcThreads = 384;  // warpgroup 0 TMA, warpgroups 1-2 MMA + epilogue
+constexpr int kTcEpiWarps = 8;
+constexpr int kTcStgCap = 256;   // staged survivors per consumer warp (8-byte key + 2-byte query index each)
+constexpr int kTcStgBytes = kTcEpiWarps * kTcStgCap * 10 + 4 * kTcEpiWarps;
 constexpr int kTcSmem = kTcStages * kTcStageBytes + 1024 /*align*/ + 8192 /*qnorm + thresholds*/ + 256 /*barriers*/ + kTcStgBytes;
+static_assert(kTcSmem <= 227 * 1024, "tc_dist_kernel must fit the 227 KB of shared memory a block may use");
 
 struct TcArgs {
   int64_t row_start;   // absolute first row of this chunk
@@ -51,7 +55,6 @@ struct TcArgs {
   int n_row_tiles;
   int n_q_tiles;
   int kb_elems;        // elements per 128-byte k-block: 32 (fp32 read as TF32) or 64 (bf16 mirror)
-  uint32_t idesc;      // UMMA instruction descriptor for the operand type
   // fused selection (D == nullptr): only entries below the query's running threshold leave the SM
   const float* thr;             // [nq] coarse k'-th best so far
   unsigned long long* cand;     // [nq x cand_cap] keys
@@ -61,16 +64,17 @@ struct TcArgs {
   int cand_cap;
 };
 
-// Survivors of the fused selection are staged per epilogue warp in shared memory and flushed once per tile.  A push
-// straight to the per-query list needs the value its global atomicAdd returns (a ~1 us round trip under contention)
-// before the warp can go on, and while the running thresholds are still loose — the first fused launches of a scan,
-// or a clustered table where whole blobs pass — those round trips, serialised per warp, were most of the launch
-// (32 K rows took 0.7 ms, 20x their MMA time).  The stage is flushed when half full and at the end of the CTA's tiles,
-// four independent global atomics per lane at a time.
+// Survivors of the fused selection are staged per consumer warp in shared memory.  A push straight to the per-query
+// list needs the value its global atomicAdd returns (a long round trip under contention) before the warp can go on,
+// and while the running thresholds are still loose — the first fused launches of a scan, or a clustered table where
+// whole blobs pass — those round trips, serialised per warp, would dominate the launch.  The stage is checked every
+// 8 queries of a thread's accumulator, flushed when half full and at the end of the CTA's tiles, four independent
+// global atomics per lane at a time.
 struct TcStage {
   unsigned long long* key;  // [kTcStgCap]
   unsigned short* q;        // [kTcStgCap]
   int* cnt;
+  const float* qn;          // |q|^2 per query of the batch (shared memory)
 };
 
 __device__ __forceinline__ void cand_push_global(const TcArgs& a, int q, unsigned long long key) {
@@ -107,137 +111,176 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm,
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(c0), "r"(c1), "r"(bar)
       : "memory");
 }
-// K-major, 128-byte-swizzled operand tile: rows of 128 bytes, 8-row groups 1024 bytes apart (SBO), descriptor
-// version 1 (Blackwell), layout type 2 = SWIZZLE_128B (cute/arch/mma_sm100_desc.hpp SmemDescriptor).
-__device__ __forceinline__ uint64_t umma_desc(uint32_t saddr) {
+// K-major, 128-byte-swizzled operand tile: rows of 128 bytes, 8-row groups 1024 bytes apart (stride byte offset),
+// layout type 1 = SWIZZLE_128B (wgmma matrix descriptor, PTX ISA "Matrix Descriptor Format").  Every operand base is
+// 1024-byte aligned, so the base-offset field stays 0.
+__device__ __forceinline__ uint64_t gmma_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFF) >> 4);        // start address, 16-byte units
   d |= static_cast<uint64_t>(1) << 16;                        // leading byte offset (unused for swizzled K-major)
   d |= static_cast<uint64_t>(1024 >> 4) << 32;                // stride byte offset = 8 rows * 128 B
-  d |= static_cast<uint64_t>(1) << 46;                        // version = 1
-  d |= static_cast<uint64_t>(2) << 61;                        // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;                        // SWIZZLE_128B
   return d;
 }
-// kind::tf32, fp32 accumulate, A and B K-major, M = 128, N = 256 (InstrDescriptor bit layout, same header).
-__host__ __device__ __forceinline__ uint32_t umma_idesc(uint32_t fmt /* 2 = TF32, 1 = BF16 */) {
-  uint32_t d = 0;
-  d |= 1u << 4;                      // c_format = F32
-  d |= fmt << 7;                     // a_format
-  d |= fmt << 10;                    // b_format
-  d |= (kTcBN >> 3) << 17;           // n_dim
-  d |= (kTcBM >> 4) << 24;           // m_dim
-  return d;
-}
-template <bool BF16>
-__device__ __forceinline__ void umma_issue(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if (BF16) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-    return;
-  }
+// D[64 x 256] (+)= A[64 x K] * B[256 x K]^T, both K-major in shared memory; K = 8 (tf32) or 16 (bf16).
+__device__ __forceinline__ void wgmma_tf32(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n"
       ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+      "}, %128, %129, p, 1, 1;\n"
+      "}\n"
+      :
+        "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// one warp reads its 32 TMEM lanes x 32 fp32 columns (asynchronous until tmem_ld_wait)
-__device__ __forceinline__ void tmem_ld32(uint32_t (&v)[32], uint32_t taddr) {
+__device__ __forceinline__ void wgmma_bf16(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr));
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %130, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+      "}, %128, %129, p, 1, 1, 0, 0;\n"
+      "}\n"
+      :
+        "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads or writes across the asynchronous MMAs
+__device__ __forceinline__ void acc_fence(float (&d)[128]) {
+#pragma unroll
+  for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 
-// Epilogue work on one 32-column chunk of the accumulator (v[j] = dot(row, query q0+j) for this thread's row).
-__device__ __forceinline__ void epi_chunk(const TcArgs& a, const uint32_t (&v)[32], int q0, bool row_ok, float xn, int64_t i,
-                                          int64_t row_abs, const float* thr_s, const float* qn_s, const TcStage& st) {
+// One fused-mode survivor (t = m*dot + |x|^2 passed the query's threshold): the coarse distance goes to the warp's stage.
+__device__ __forceinline__ void stage_push(const TcArgs& a, const TcStage& st, int q, float t, int64_t row_abs) {
+  float d = t;
+  if (a.metric == EPS_METRIC_L2) d = fmaxf(d + st.qn[q], 0.f);
+  else if (a.metric == EPS_METRIC_COSINE) d = 1.0f + d;
+  const unsigned long long key = make_key(d, static_cast<uint32_t>(row_abs));
+  const int pos = atomicAdd(st.cnt, 1);  // shared memory
+  if (pos < kTcStgCap) { st.key[pos] = key; st.q[pos] = static_cast<unsigned short>(q); }
+  else cand_push_global(a, q, key);      // stage full (flushed at the next check)
+}
+
+// Epilogue of one 64 x 256 accumulator.  This thread holds rows r[h] (h = 0, 1: acc[4j + 2h + c]) and queries
+// qc + 8j + c (j < 32, c = 0, 1) — the wgmma fp32 accumulator fragment.
+__device__ __forceinline__ void epilogue(const TcArgs& a, const float (&acc)[128], int qc, const bool (&row_ok)[2],
+                                         const float (&xn)[2], const int64_t (&i)[2], const int64_t (&row_abs)[2],
+                                         const float* thr_s, const float* qn_s, const TcStage& st, int lane) {
   if (a.D == nullptr) {
     // ---- fused selection: 2 instructions per element (FFMA + compare), survivors are rare ----
-    if (row_ok) {
-      const float m = a.metric == EPS_METRIC_L2 ? -2.0f : -1.0f;
+    const float m = a.metric == EPS_METRIC_L2 ? -2.0f : -1.0f;
 #pragma unroll
-      for (int j4 = 0; j4 < 8; ++j4) {
-        const float4 ct = *reinterpret_cast<const float4*>(thr_s + q0 + 4 * j4);
-        const float t0 = fmaf(m, __uint_as_float(v[4 * j4 + 0]), xn), t1 = fmaf(m, __uint_as_float(v[4 * j4 + 1]), xn);
-        const float t2 = fmaf(m, __uint_as_float(v[4 * j4 + 2]), xn), t3 = fmaf(m, __uint_as_float(v[4 * j4 + 3]), xn);
-        if ((t0 < ct.x) | (t1 < ct.y) | (t2 < ct.z) | (t3 < ct.w)) {
-          const float tt[4] = {t0, t1, t2, t3};
-          const float cc[4] = {ct.x, ct.y, ct.z, ct.w};
+    for (int g = 0; g < 8; ++g) {
 #pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            if (tt[u] < cc[u]) {
-              const int q = q0 + 4 * j4 + u;
-              float d = tt[u];
-              if (a.metric == EPS_METRIC_L2) d = fmaxf(d + qn_s[q], 0.f);
-              else if (a.metric == EPS_METRIC_COSINE) d = 1.0f + d;
-              const unsigned long long key = make_key(d, static_cast<uint32_t>(row_abs));
-              const int pos = atomicAdd(st.cnt, 1);  // shared memory
-              if (pos < kTcStgCap) { st.key[pos] = key; st.q[pos] = static_cast<unsigned short>(q); }
-              else cand_push_global(a, q, key);      // stage full (flushed at the next chunk boundary)
-            }
+      for (int jj = 0; jj < 4; ++jj) {
+        const int j = 4 * g + jj;
+        const float2 ct = *reinterpret_cast<const float2*>(thr_s + qc + 8 * j);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float t0 = fmaf(m, acc[4 * j + 2 * h], xn[h]), t1 = fmaf(m, acc[4 * j + 2 * h + 1], xn[h]);
+          if (row_ok[h] && ((t0 < ct.x) | (t1 < ct.y))) {
+            if (t0 < ct.x) stage_push(a, st, qc + 8 * j, t0, row_abs[h]);
+            if (t1 < ct.y) stage_push(a, st, qc + 8 * j + 1, t1, row_abs[h]);
           }
         }
       }
+      __syncwarp();
+      if (*st.cnt >= kTcStgCap / 2) cand_flush(a, st, lane);
     }
   } else {
     // ---- distance tile to global memory (first chunk: seeds the running thresholds) ----
 #pragma unroll
     for (int j = 0; j < 32; ++j) {
-      const int q = q0 + j;
-      if (row_ok && q < a.nq) {
-        const float dot = __uint_as_float(v[j]);
-        float d;
-        if (a.metric == EPS_METRIC_L2) d = fmaxf(xn + qn_s[q] - 2.0f * dot, 0.f);
-        else if (a.metric == EPS_METRIC_COSINE) d = 1.0f - dot;
-        else d = -dot;
-        a.D[static_cast<int64_t>(q) * a.ldd + i] = d;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const int q = qc + 8 * j + c;
+          if (row_ok[h] && q < a.nq) {
+            const float dot = acc[4 * j + 2 * h + c];
+            float d;
+            if (a.metric == EPS_METRIC_L2) d = fmaxf(xn[h] + qn_s[q] - 2.0f * dot, 0.f);
+            else if (a.metric == EPS_METRIC_COSINE) d = 1.0f - dot;
+            else d = -dot;
+            a.D[static_cast<int64_t>(q) * a.ldd + i[h]] = d;
+          }
+        }
       }
     }
   }
 }
 
+template <bool BF16>
 __global__ void __launch_bounds__(kTcThreads, 1) tc_dist_kernel(const __grid_constant__ CUtensorMap tmA,
                                                               const __grid_constant__ CUtensorMap tmB, TcArgs a) {
   extern __shared__ unsigned char tc_smem_raw[];
   // 1024-byte alignment for the 128-byte swizzle pattern
   unsigned char* base = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~uintptr_t(1023));
   float* qn_s = reinterpret_cast<float*>(base + kTcStages * kTcStageBytes);  // [<=1024]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(base + kTcStages * kTcStageBytes + 8192);
-  // bars[0..3] full, [4..7] empty, [8..9] tmem_full, [10..11] tmem_empty, then the TMEM base slot
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 12);
-  unsigned char* stg = base + kTcStages * kTcStageBytes + 8192 + 256;  // [4 x keys][4 x query indices][4 counters]
-  const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + 4), tfull0 = smem_u32(bars + 8), tempty0 = smem_u32(bars + 10);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(base + kTcStages * kTcStageBytes + 8192);  // [0..3] full, [4..7] empty
+  unsigned char* stg = base + kTcStages * kTcStageBytes + 8192 + 256;  // [8 x keys][8 x query indices][8 counters]
+  const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + kTcStages);
   const uint32_t stage0 = smem_u32(base);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nkb = (a.dim + a.kb_elems - 1) / a.kb_elems;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kTcStages; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, 1); }
-    for (int t = 0; t < 2; ++t) { mbar_init(tfull0 + 8 * t, 1); mbar_init(tempty0 + 8 * t, 4); }
+    for (int s = 0; s < kTcStages; ++s) { mbar_init(full0 + 8 * s, 1); mbar_init(empty0 + 8 * s, kTcEpiWarps); }
     mbar_fence_init();
-  }
-  if (warp == 1) {  // TMEM: all 512 columns (two 256-column fp32 accumulators)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_slot)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   float* thr_s = qn_s + 1024;  // [<=1024] thresholds (fused mode)
   // fused mode compares t = m*dot + xn (m = -2 for L2, -1 otherwise) with a per-query constant:
@@ -253,15 +296,13 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dist_kernel(const __grid_con
     }
     thr_s[i] = c;
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
 
   const int tiles_per_row = a.n_q_tiles;
-  if (warp == 0) {
-    // ===== TMA producer =====
-    if (lane == 0) {
+  if (warp < 4) {
+    // ===== TMA producer (warpgroup 0; gives its registers to the consumers) =====
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (threadIdx.x == 0) {
       asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmA)) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&tmB)) : "memory");
       uint32_t it = 0;
@@ -279,82 +320,63 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dist_kernel(const __grid_con
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      const bool bf16 = a.kb_elems == 64;
-      const uint32_t idesc = bf16 ? umma_idesc(1u) : umma_idesc(2u);
-      uint32_t it = 0, tc = 0;
-      for (int rt = blockIdx.x; rt < a.n_row_tiles; rt += gridDim.x) {
-        for (int qt = 0; qt < tiles_per_row; ++qt, ++tc) {
-          const uint32_t acc = tc & 1, aph = (tc >> 1) & 1;
-          mbar_wait(tempty0 + 8 * acc, aph ^ 1);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t tmem_d = tmem_base + acc * kTcBN;
-          for (int kb = 0; kb < nkb; ++kb, ++it) {
-            const uint32_t s = it % kTcStages, ph = (it / kTcStages) & 1;
-            mbar_wait(full0 + 8 * s, ph);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t sa = stage0 + s * kTcStageBytes;
-            const uint64_t ad = umma_desc(sa), bd = umma_desc(sa + kTcABytes);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {  // 4 MMAs per 128-byte block: K = 8 tf32 / 16 bf16 = 32 bytes = +2 (16-B units)
-              if (bf16) umma_issue<true>(tmem_d, ad + 2 * k, bd + 2 * k, idesc, (kb | k) ? 1u : 0u);
-              else umma_issue<false>(tmem_d, ad + 2 * k, bd + 2 * k, idesc, (kb | k) ? 1u : 0u);
-            }
-            umma_commit(empty0 + 8 * s);  // frees the stage when these MMAs retire
-          }
-          umma_commit(tfull0 + 8 * acc);  // accumulator complete
-        }
-      }
-    }
   } else {
-    // ===== epilogue: warps 2..5 own TMEM lanes 32*(warp%4) .. +31 =====
-    const int lq = (warp & 3) * 32;
+    // ===== consumers: warpgroup 1 + cw owns rows 64*cw .. +63 of every tile, warp (warp & 3) 16 of them =====
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+    const int cw = (warp >> 2) - 1, ew = warp - 4;
     TcStage st;
-    st.key = reinterpret_cast<unsigned long long*>(stg) + (warp & 3) * kTcStgCap;
-    st.q = reinterpret_cast<unsigned short*>(stg + 4 * kTcStgCap * 8) + (warp & 3) * kTcStgCap;
-    st.cnt = reinterpret_cast<int*>(stg + 4 * kTcStgCap * 10) + (warp & 3);
+    st.key = reinterpret_cast<unsigned long long*>(stg) + ew * kTcStgCap;
+    st.q = reinterpret_cast<unsigned short*>(stg + kTcEpiWarps * kTcStgCap * 8) + ew * kTcStgCap;
+    st.cnt = reinterpret_cast<int*>(stg + kTcEpiWarps * kTcStgCap * 10) + ew;
+    st.qn = qn_s;
     if (lane == 0) *st.cnt = 0;
     __syncwarp();
-    uint32_t tc = 0;
+    const int r_lo = 64 * cw + 16 * (warp & 3) + (lane >> 2);  // tile row of acc[4j + 0..1]; acc[4j + 2..3]: r_lo + 8
+    float acc[128];
+#pragma unroll
+    for (int v = 0; v < 128; ++v) acc[v] = 0.f;
+    uint32_t it = 0;
     for (int rt = blockIdx.x; rt < a.n_row_tiles; rt += gridDim.x) {
-      const int64_t i = static_cast<int64_t>(rt) * kTcBM + lq + lane;  // row index inside the chunk
-      bool row_ok = i < a.n;
-      float xn = 0.f;
-      if (a.metric == EPS_METRIC_L2 && row_ok) xn = a.xnorm[a.row_start + i];
-      const int64_t row_abs = a.row_start + i;
-      if (a.D == nullptr && a.pass && row_ok) {
-        const int64_t pi = row_abs - a.pass_base;
-        row_ok = (a.pass[pi >> 5] >> (pi & 31)) & 1u;
-      }
-      for (int qt = 0; qt < tiles_per_row; ++qt, ++tc) {
-        const uint32_t acc = tc & 1, aph = (tc >> 1) & 1;
-        mbar_wait(tfull0 + 8 * acc, aph);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t taddr0 = tmem_base + (static_cast<uint32_t>(lq) << 16) + acc * kTcBN;
-        const int qbase = qt * kTcBN;
-#pragma unroll 1
-        for (int c = 0; c < kTcBN / 32; ++c) {
-          uint32_t v[32];
-          tmem_ld32(v, taddr0 + c * 32);
-          tmem_ld_wait();
-          epi_chunk(a, v, qbase + c * 32, row_ok, xn, i, row_abs, thr_s, qn_s, st);
-          if (a.D == nullptr) {
-            __syncwarp();
-            if (*st.cnt >= kTcStgCap / 2) cand_flush(a, st, lane);
-          }
+      bool row_ok[2];
+      float xn[2];
+      int64_t i[2], row_abs[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        i[h] = static_cast<int64_t>(rt) * kTcBM + r_lo + 8 * h;  // row index inside the chunk
+        row_ok[h] = i[h] < a.n;
+        xn[h] = (a.metric == EPS_METRIC_L2 && row_ok[h]) ? a.xnorm[a.row_start + i[h]] : 0.f;
+        row_abs[h] = a.row_start + i[h];
+        if (a.D == nullptr && a.pass && row_ok[h]) {
+          const int64_t pi = row_abs[h] - a.pass_base;
+          row_ok[h] = (a.pass[pi >> 5] >> (pi & 31)) & 1u;
         }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
+      }
+      for (int qt = 0; qt < tiles_per_row; ++qt) {
+        uint32_t prev = 0;
+        for (int kb = 0; kb < nkb; ++kb, ++it) {
+          const uint32_t s = it % kTcStages, ph = (it / kTcStages) & 1;
+          mbar_wait(full0 + 8 * s, ph);
+          const uint32_t sa = stage0 + s * kTcStageBytes;
+          const uint64_t ad = gmma_desc(sa + cw * (kTcABytes / 2)), bd = gmma_desc(sa + kTcABytes);
+          wgmma_fence();
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {  // 4 MMAs per 128-byte block: K = 8 tf32 / 16 bf16 = 32 bytes = +2 (16-B units)
+            if (BF16) wgmma_bf16(acc, ad + 2 * k, bd + 2 * k, (kb | k) ? 1u : 0u);
+            else wgmma_tf32(acc, ad + 2 * k, bd + 2 * k, (kb | k) ? 1u : 0u);
+          }
+          wgmma_commit();
+          wgmma_wait<1>();  // the previous block's MMAs have retired: its stage can be refilled
+          if (kb > 0 && lane == 0) mbar_arrive(empty0 + 8 * prev);
+          prev = s;
+        }
+        wgmma_wait<0>();
+        acc_fence(acc);
+        if (lane == 0) mbar_arrive(empty0 + 8 * prev);
+        epilogue(a, acc, qt * kTcBN + 2 * (lane & 3), row_ok, xn, i, row_abs, thr_s, qn_s, st, lane);
+        acc_fence(acc);
       }
     }
     if (a.D == nullptr) cand_flush(a, st, lane);  // what is left in the stage (it is also flushed whenever half full)
-  }
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
   }
 }
 
@@ -478,7 +500,6 @@ int tc_launch_distances(Index* ix, int64_t row_start, int64_t n, const float* d_
   a.row_start = row_start; a.n = n; a.nq = nq; a.ldd = ldd;
   a.xnorm = ix->s_xnorm.as<float>(); a.qnorm = ix->s_qnorm.as<float>(); a.D = D; a.dim = dim; a.metric = ix->metric;
   a.kb_elems = bf16 ? 64 : 32;
-  a.idesc = umma_idesc(bf16 ? 1u : 2u);
   a.thr = nullptr; a.cand = nullptr; a.cand_cnt = nullptr; a.pass = nullptr; a.pass_base = 0; a.cand_cap = 0;
   if (fused) {
     a.D = nullptr;
@@ -489,11 +510,13 @@ int tc_launch_distances(Index* ix, int64_t row_start, int64_t n, const float* d_
   a.n_q_tiles = static_cast<int>((nq + kTcBN - 1) / kTcBN);
   static bool attr_set = false;
   if (!attr_set) {
-    EPS_CUDA(cudaFuncSetAttribute(tc_dist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmem));
+    EPS_CUDA(cudaFuncSetAttribute(tc_dist_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmem));
+    EPS_CUDA(cudaFuncSetAttribute(tc_dist_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmem));
     attr_set = true;
   }
   const int grid = std::min(a.n_row_tiles, ix->num_sms);
-  tc_dist_kernel<<<grid, kTcThreads, kTcSmem, ix->stream>>>(tmA, tmB, a);
+  if (bf16) tc_dist_kernel<true><<<grid, kTcThreads, kTcSmem, ix->stream>>>(tmA, tmB, a);
+  else tc_dist_kernel<false><<<grid, kTcThreads, kTcSmem, ix->stream>>>(tmA, tmB, a);
   EPS_CUDA(cudaGetLastError());
   ++*launches;
   return EPS_OK;

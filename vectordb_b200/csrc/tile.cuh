@@ -7,6 +7,31 @@ namespace eps {
 
 constexpr int kC = 128;  // candidate slots per vertex
 
+__device__ __forceinline__ uint32_t mix32(uint32_t x) {
+  x ^= x >> 16; x *= 0x7feb352dU; x ^= x >> 15; x *= 0x846ca68bU; x ^= x >> 16;
+  return x;
+}
+
+// Bounded reverse lists that do not depend on arrival order: list p keeps the `cap` arrivals v with the smallest
+// key (mix32 priority, v), in key order.  Each push runs an atomicMin cascade down the slots (a slot keeps the smaller
+// of its key and the incoming one and passes the larger on), so slot i ends as the i-th smallest key pushed whatever
+// the interleaving.  Slots start at kRevEmpty; cnt[p] counts every arrival.
+constexpr unsigned long long kRevEmpty = ~0ull;
+__device__ __forceinline__ void rev_push(unsigned long long* __restrict__ slots, int cap, int32_t* __restrict__ cnt,
+                                         int32_t p, int32_t v, uint32_t salt) {
+  atomicAdd(&cnt[p], 1);
+  unsigned long long* s = slots + static_cast<int64_t>(p) * cap;
+  unsigned long long x = (static_cast<unsigned long long>(mix32(static_cast<uint32_t>(v) * 0x9E3779B1u ^ salt)) << 32) |
+                         static_cast<uint32_t>(v);
+  if (*reinterpret_cast<volatile unsigned long long*>(s + cap - 1) <= x) return;  // the last kept key only ever drops
+  for (int i = 0; i < cap; ++i) {
+    const unsigned long long old = atomicMin(s + i, x);
+    if (old == kRevEmpty) return;
+    x = old > x ? old : x;
+  }
+}
+__device__ __forceinline__ int32_t rev_id(unsigned long long key) { return static_cast<int32_t>(static_cast<uint32_t>(key)); }
+
 // cand [batch x kC] row ids (-1 = empty).  D [batch x kC x kC] = L2^2 between candidate rows.
 template <bool L2, bool VEC4>
 __global__ void __launch_bounds__(256) pair_tile_kernel(const float* __restrict__ vectors, int dim, int metric,

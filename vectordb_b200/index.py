@@ -128,7 +128,7 @@ class Index:
         check(self.L.eps_index_set_graph_tuning(self.h, int(ring_slots), int(ctas_per_sm)))
 
     def set_coarse(self, mode):
-        """0 = fp32 SIMT only, 1 = tcgen05 TF32 (default), 2 = tcgen05 bf16 mirror (exact re-score in all modes)."""
+        """0 = fp32 SIMT only, 1 = wgmma TF32 (default), 2 = wgmma bf16 mirror (exact re-score in all modes)."""
         check(self.L.eps_index_set_coarse(self.h, {"fp32": 0, "tf32": 1, "bf16": 2}.get(mode, mode)))
 
     def set_coarse_guard(self, on=True):

@@ -50,7 +50,7 @@ def library_path():
 
 
 def build_library(verbose=False):
-    """Compile csrc/ for sm_100a in-tree (nvcc cross-compiles without a GPU)."""
+    """Compile csrc/ for sm_90a in-tree (nvcc cross-compiles without a GPU)."""
     out = None if verbose else subprocess.DEVNULL
     subprocess.check_call(["make", "-C", os.path.join(HERE, "csrc"), "-j8"], stdout=out)
 

@@ -54,7 +54,8 @@ constexpr int kMaxR = 24;       // ring slots (upper bound: 3 consumer warps x k
 constexpr int kRounds = kMaxW * kEll / kGsThreads;  // adjacency slots per thread
 
 // Developer build only (make EXTRA=-DEPS_GS_PROFILE): per-phase cycle counters of warp 0 (pick / adjacency / merge /
-// barrier waits) and of warp 1 (row wait / row math), summed over CTAs into stats[8..15].  Compiled out otherwise.
+// barrier waits) and of warp 1 (row wait / row math), summed over CTAs into stats[8..23], and the prefix-rejection
+// counts of prof_prefix_fails in stats[25..29].  Compiled out otherwise.
 #ifdef EPS_GS_PROFILE
 #define GS_T(var) const long long var = clock64()
 #define GS_ACC(slot, t0, t1) do { if (lane == 0) prof[slot] += (t1) - (t0); } while (0)
@@ -147,12 +148,45 @@ __device__ __forceinline__ void warp_rows_scalar(const float* const (&rows)[S], 
   for (int s = 0; s < S; ++s) out[s] = warp_sum(acc[s]);
 }
 
+#ifdef EPS_GS_PROFILE
+// Developer build: could a prefix of a staged L2 row reject it before the rest is read?  For t = dim4 * j / 4 float4
+// chunks (j = 1..4; j = 4 is the whole row), cnt[j] counts the rows of `mask` whose prefix already fails the bound.  The
+// test is the exact one a prefix rejection would need: lane l's chain over its chunks l, l + 32, ... below t is an
+// intermediate value of its full fmaf chain, each step adds a square >= 0, so lane s's butterfly of the partial chains
+// is <= its distance of row s, and a partial key >= bound proves that the full key fails too.  A second pass over the
+// rows in shared memory: the distances the search uses are untouched.
+template <int S>
+__device__ __forceinline__ void prof_prefix_fails(const unsigned char* first, uint32_t step, unsigned mask, const float4* q, int dim4,
+                                                  int lane, const int* slot_id, int cw, unsigned long long bound,
+                                                  unsigned long long* cnt) {
+  if (lane < S && ((mask >> lane) & 1u)) ++cnt[0];
+  for (int j = 1; j <= 4; ++j) {
+    const int t = dim4 * j / 4;
+    float acc[S];
+#pragma unroll
+    for (int s = 0; s < S; ++s) acc[s] = 0.f;
+    for (int c = lane; c < t; c += 32) {
+      const float4 y = q[c];
+#pragma unroll
+      for (int s = 0; s < S; ++s)
+        if ((mask >> s) & 1u) acc4<true>(reinterpret_cast<const float4*>(first + s * step)[c], y, acc[s]);
+    }
+#pragma unroll
+    for (int s = 0; s < S; ++s) {
+      const float v = warp_sum(acc[s]);
+      if (lane == s && ((mask >> s) & 1u) && make_key(v, static_cast<uint32_t>(slot_id[cw + 3 * s])) >= bound) ++cnt[j];
+    }
+  }
+}
+#endif
+
 // Consumer step of one warp over its S slots (slot of local index s = cw + 3 s): wait for the landed rows, distances,
 // accepted keys to the pending buffer.  Returns nothing; the caller refills the slots.
 template <int S>
 __device__ __forceinline__ void consume_slots(const GSArgs& a, unsigned occ_mask, unsigned par_mask, int cw, int lane, bool staged,
                                               const unsigned char* ring, uint32_t bar0, const float* qv, const int* slot_id,
-                                              unsigned long long bound, unsigned long long* pend, int* s_npend) {
+                                              unsigned long long bound, unsigned long long* pend, int* s_npend,
+                                              unsigned long long* prefix_cnt) {
   float d[S];
   if (staged) {
 #pragma unroll
@@ -162,6 +196,10 @@ __device__ __forceinline__ void consume_slots(const GSArgs& a, unsigned occ_mask
     const uint32_t step = 3u * static_cast<uint32_t>(a.slot_bytes);
     if (a.metric == EPS_METRIC_L2) warp_rows_vec4<true, S>(first, step, occ_mask, reinterpret_cast<const float4*>(qv), a.dim >> 2, lane, d);
     else warp_rows_vec4<false, S>(first, step, occ_mask, reinterpret_cast<const float4*>(qv), a.dim >> 2, lane, d);
+#ifdef EPS_GS_PROFILE
+    if (a.metric == EPS_METRIC_L2)
+      prof_prefix_fails<S>(first, step, occ_mask, reinterpret_cast<const float4*>(qv), a.dim >> 2, lane, slot_id, cw, bound, prefix_cnt);
+#endif
   } else {
     const float* rows[S];
 #pragma unroll
@@ -237,7 +275,11 @@ __device__ __forceinline__ void merge_pending(unsigned long long* qa, unsigned l
   }
 }
 
-__global__ void __launch_bounds__(kGsThreads, 7) graph_search_kernel(GSArgs a) {
+// Two register budgets of the same kernel: 72 registers per thread allow 7 resident CTAs per SM but spill 452 B per
+// thread to local memory (1320 B of spill loads); 128 registers allow 4 and spill 60 B (72 B of loads).  graph_search
+// picks the instance from the geometry it launches.
+template <int kMinCtas>
+__global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSArgs a) {
   extern __shared__ __align__(128) unsigned char gs_smem[];
   const int dim4p = (a.dim + 3) & ~3;
   unsigned char* ring = gs_smem;                                                                   // [R][slot_bytes]
@@ -281,6 +323,9 @@ __global__ void __launch_bounds__(kGsThreads, 7) graph_search_kernel(GSArgs a) {
 #ifdef EPS_GS_PROFILE
   long long prof[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // 0 barrier X, 1 merge, 2 row wait, 3 row math, 4 pick, 5 barrier 1, 6 adjacency+visited, 7 barrier 2 + FIFO
   const long long t_kernel0 = clock64();
+  unsigned long long prefix_cnt[5] = {0, 0, 0, 0, 0};  // staged L2 rows evaluated; of them, rows whose 1/4 .. 4/4 prefix fails the bound
+#else
+  unsigned long long* prefix_cnt = nullptr;
 #endif
 
   for (;;) {
@@ -352,10 +397,10 @@ __global__ void __launch_bounds__(kGsThreads, 7) graph_search_kernel(GSArgs a) {
         for (;;) {
           if (occ_mask) {
             GS_T(tw0);
-            if (n_own <= 1) consume_slots<1>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend);
-            else if (n_own <= 2) consume_slots<2>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend);
-            else if (n_own <= 4) consume_slots<4>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend);
-            else consume_slots<8>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend);
+            if (n_own <= 1) consume_slots<1>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend, prefix_cnt);
+            else if (n_own <= 2) consume_slots<2>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend, prefix_cnt);
+            else if (n_own <= 4) consume_slots<4>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend, prefix_cnt);
+            else consume_slots<8>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend, prefix_cnt);
             par_mask ^= occ_mask;
             GS_T(tw1);
             GS_ACC(3, tw0, tw1);
@@ -582,6 +627,7 @@ __global__ void __launch_bounds__(kGsThreads, 7) graph_search_kernel(GSArgs a) {
     for (int i = 0; i < 8; ++i) atomicAdd(&a.stats[8 + warp * 8 + i], static_cast<unsigned long long>(prof[i]));
     if (warp == 0) atomicAdd(&a.stats[24], static_cast<unsigned long long>(clock64() - t_kernel0));
   }
+  for (int i = 0; i < 5; ++i) if (prefix_cnt[i]) atomicAdd(&a.stats[25 + i], prefix_cnt[i]);
 #endif
   if (st_ndist) atomicAdd(&a.stats[0], st_ndist);
   if (st_nexp) atomicAdd(&a.stats[1], st_nexp);
@@ -693,9 +739,10 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   };
   while (R > 2 && smem_for(R) > 200 * 1024) --R;
   if (smem_for(R) > 226 * 1024) return fail(EPS_ERR_UNSUPPORTED, "queue + query + row ring do not fit in shared memory");
-  EPS_CUDA(cudaFuncSetAttribute(graph_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_for(R))));
+  EPS_CUDA(cudaFuncSetAttribute(graph_search_kernel<7>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_for(R))));
+  EPS_CUDA(cudaFuncSetAttribute(graph_search_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_for(R))));
   auto resident = [&](int r, int* out) {
-    EPS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(out, graph_search_kernel, kGsThreads, smem_for(r)));
+    EPS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(out, graph_search_kernel<7>, kGsThreads, smem_for(r)));
     if (*out < 1) *out = 1;
     if (ix->graph_ctas_per_sm > 0) *out = std::min(*out, ix->graph_ctas_per_sm);
     return EPS_OK;
@@ -735,7 +782,7 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
     ix->vis_clean_words = words;
     ix->vis_clean_cap = ix->s_visited.cap;
   }
-  EPS_TRY(ix->s_misc.reserve(256));  // [0..3] counters, [+32 B] work counter, [8..24] developer phase timers
+  EPS_TRY(ix->s_misc.reserve(256));  // [0..3] counters, [+32 B] work counter, [8..24] developer phase timers, [25..29] developer prefix counts
   EPS_CUDA(cudaMemsetAsync(ix->s_misc.p, 0, 256, ix->stream));
   uint64_t launches = 1;
   EPS_TRY(ensure_ell(ix, &launches));
@@ -770,7 +817,11 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   a.qtimes = ix->s_tail.as<unsigned long long>();
   ix->prof_nq = nq;
 #endif
-  graph_search_kernel<<<slots, kGsThreads, smem, ix->stream>>>(a);
+  // at most 4 resident CTAs per SM (what the auto rule picks for batches above one wave at 7 per SM, e.g. 1024 queries
+  // at L = 768): the register file has room for 128 registers per thread, so the instance that hardly spills runs;
+  // smaller batches keep 7 resident queries per SM
+  if (per_sm <= 4) graph_search_kernel<4><<<slots, kGsThreads, smem, ix->stream>>>(a);
+  else graph_search_kernel<7><<<slots, kGsThreads, smem, ix->stream>>>(a);
   EPS_CUDA(cudaGetLastError());
   if (stats) {
     stats->n_seed += static_cast<uint64_t>(nq) * static_cast<uint64_t>(L);
@@ -796,6 +847,16 @@ int read_graph_counters(Index* ix, eps_stats* stats) {
   for (int w = 0; w < 2; ++w)
     for (int i = 0; i < 8; ++i) fprintf(stderr, " w%d.%s=%.1f%%", w, names[i], 100.0 * static_cast<double>(pr[8 + w * 8 + i]) / tot);
   fprintf(stderr, "\n");
+  if (pr[25]) {
+    // fetching a prefix s of every row and the rest only where the prefix cannot reject it would stage
+    // s + (1 - p(s)) (1 - s) of the row bytes, p(s) = share of rows whose prefix s fails the bound
+    fprintf(stderr, "[gs-profile] staged L2 rows evaluated %llu; share whose prefix fails the bound (row bytes staged by a split there):", pr[25]);
+    for (int j = 1; j <= 4; ++j) {
+      const double p = static_cast<double>(pr[25 + j]) / static_cast<double>(pr[25]), s = 0.25 * j;
+      fprintf(stderr, " %d/4 %.4f (%.4f)", j, p, s + (1.0 - p) * (1.0 - s));
+    }
+    fprintf(stderr, "\n");
+  }
   if (ix->prof_nq > 0 && ix->s_tail.p) {
     std::vector<unsigned long long> t(static_cast<size_t>(ix->prof_nq) * 4);
     EPS_CUDA(cudaMemcpy(t.data(), ix->s_tail.p, t.size() * 8, cudaMemcpyDeviceToHost));

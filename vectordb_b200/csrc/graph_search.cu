@@ -19,8 +19,8 @@
 //   * the sorted queue (L 64-bit keys), the query vector, a FIFO of fresh neighbour ids and a RING of row
 //     slots live in shared memory;
 //   * a neighbour row is brought HBM -> shared memory by ONE 1-D bulk async copy (TMA engine,
-//     cp.async.bulk + mbarrier complete_tx) issued by a single lane: no registers are held across the wait,
-//     every free ring slot is in flight at once, and the adjacency reads + visited-bitmap atomics of the NEXT
+//     cp.async.bulk + mbarrier complete_tx, L2 evict_first) issued by a single lane: no registers are held across the wait,
+//     every free ring slot is in flight at once, and the adjacency reads + visited tests of the NEXT
 //     candidates run while the rows of the previous ones land;
 //   * distances: warps 1-3 own the ring slots (slot s <-> warp 1 + s % 3); a warp waits on the mbarriers of its
 //     occupied slots, evaluates up to 8 landed rows with all 32 lanes on every row (float4 from shared memory, the
@@ -28,9 +28,12 @@
 //     while the FIFO has a backlog; accepted keys (key < worst-in-queue) go to a small pending buffer that is merged
 //     into the sorted queue by a block-parallel rank-and-shift, at the latest when the expansion is consumed;
 //   * adjacency: fixed-stride rows of 64 int32 ids (one 256-byte read from the vertex id; longer rows
-//     continue in the CSR); visited: one bitmap per in-flight query in global memory, atomicOr test-and-set,
-//     cleared by the CTA after the query like the reference clears its vector<bool> (:711-714) — on large tables
-//     only the words the query touched, from a log of its fresh ids.
+//     continue in the CSR); visited: a per-slot open-addressing hash set of int32 ids in global memory (16 L entries,
+//     at most 64 KB: the tables of all resident queries fit in L2), one 32-byte bucket read + atomicCAS per
+//     test-and-insert, refilled with 0xFF after the query like the reference clears its vector<bool> (:711-714).  A
+//     query that would fill the set beyond 3/4 moves to a bitmap of n bits (atomicOr test-and-set) for the rest of
+//     its run; that bitmap is cleared after the query — on large tables only the words the query touched, from a log
+//     of its fresh ids.
 // every iteration picks up to W (the search width) unchecked candidates, and the next pick waits until all their rows
 //   are consumed and merged.  Width 1 has the visit order, results and distance-evaluation counts of the reference
 //   at IntraQueryThreads = 1; widths 2..8 expand W candidates together — the device analogue of IntraQueryThreads > 1,
@@ -72,12 +75,16 @@ struct GSArgs {
   const int32_t* init_ids;
   const float* seed_dist;         // [nq x seed_ld] distances of the seed set (dense tile product)
   const float* queries;
-  uint32_t* visited;              // [slots x visited_words]
-  int32_t* vlog;                  // [slots x vlog_cap] ids whose bit the running query has set, in FIFO order (visited reset)
+  uint32_t* vset;                 // [slots x vset_cap] hash set of the ids the running query has visited (kVsetEmpty = free)
+  int vset_cap;                   // entries per slot: a power of two >= 1024
+  int vset_shift;                 // bucket of an id = (id * kVsetMul) >> vset_shift, 8 entries per bucket
+  int vset_max;                   // entries a query may insert before it moves to the bitmap (3/4 of vset_cap)
+  uint32_t* visited;              // [slots x visited_words] bitmaps of the queries that outgrew their hash set
+  int32_t* vlog;                  // [slots x vlog_cap] the running query's fresh ids in FIFO order (migration, bitmap reset)
   int vlog_cap;
   unsigned long long* out_queue;  // [nq x L]
   int* work_counter;
-  unsigned long long* stats;      // n_dist, n_expand, n_edges
+  unsigned long long* stats;      // n_dist, n_expand, n_edges (+ developer counters, see read_graph_counters)
   int64_t visited_words;
   int64_t seed_ld;
   int dim, metric, vec4;
@@ -97,6 +104,27 @@ __device__ __forceinline__ int lb_masked(const unsigned long long* a, int n, uns
     if ((a[mid] & kKeyMask) < key) lo = mid + 1; else hi = mid;
   }
   return lo;
+}
+
+// Visited hash set: linear probing over the entries of a slot's table from the first entry of the id's bucket
+// (multiplicative hash).  Entries go from kVsetEmpty to an id once and stay until the table is refilled after the
+// query, so an id found anywhere is visited, and an entry seen holding another id stays so.  Reads bypass L1
+// (__ldcg): the entries are written by L2 atomics.
+constexpr uint32_t kVsetEmpty = 0xffffffffu;  // ids are < 2^31
+constexpr uint32_t kVsetMul = 0x9e3779b1u;
+__device__ __forceinline__ uint32_t vset_bucket(uint32_t id, int shift) { return ((id * kVsetMul) >> shift) << 3; }
+// Test-and-insert from entry p on, one atomicCAS per entry: true when the id was absent (this thread inserted it).
+// Terminates because a query never fills its table beyond 3/4.  `acc` counts table accesses (developer build).
+__device__ __forceinline__ bool vset_claim(uint32_t* t, uint32_t mask, uint32_t p, uint32_t id, unsigned long long& acc) {
+  for (;;) {
+    const uint32_t old = atomicCAS(t + p, kVsetEmpty, id);
+#ifdef EPS_GS_PROFILE
+    ++acc;
+#endif
+    if (old == kVsetEmpty) return true;
+    if (old == id) return false;
+    p = (p + 1) & mask;
+  }
 }
 
 template <bool L2>
@@ -275,8 +303,8 @@ __device__ __forceinline__ void merge_pending(unsigned long long* qa, unsigned l
   }
 }
 
-// Two register budgets of the same kernel: 72 registers per thread allow 7 resident CTAs per SM but spill 452 B per
-// thread to local memory (1320 B of spill loads); 128 registers allow 4 and spill 60 B (72 B of loads).  graph_search
+// Two register budgets of the same kernel: 72 registers per thread allow 7 resident CTAs per SM but spill 376 B per
+// thread to local memory (348 B of spill loads); 128 registers allow 4 and spill 12 B (16 B of loads).  graph_search
 // picks the instance from the geometry it launches.
 template <int kMinCtas>
 __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSArgs a) {
@@ -308,8 +336,11 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
   const bool staged = a.slot_bytes > 0;
   const uint32_t ring0 = smem_u32(ring), bar0 = smem_u32(bars);
   const uint32_t row_bytes = static_cast<uint32_t>(a.dim) * 4u;
+  uint32_t* vset = a.vset + static_cast<int64_t>(blockIdx.x) * a.vset_cap;
+  const uint32_t vmask = static_cast<uint32_t>(a.vset_cap) - 1u;
   uint32_t* visited = a.visited + static_cast<int64_t>(blockIdx.x) * a.visited_words;
   int32_t* vlog = a.vlog + static_cast<int64_t>(blockIdx.x) * a.vlog_cap;
+  unsigned long long vacc = 0;  // developer build: hash-set accesses (bucket reads + CAS) of this thread
 
   if (tid == 0) {
     for (int s = 0; s < R; ++s) mbar_init(bar0 + 8 * s, 1);
@@ -324,6 +355,7 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
   long long prof[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // 0 barrier X, 1 merge, 2 row wait, 3 row math, 4 pick, 5 barrier 1, 6 adjacency+visited, 7 barrier 2 + FIFO
   const long long t_kernel0 = clock64();
   unsigned long long prefix_cnt[5] = {0, 0, 0, 0, 0};  // staged L2 rows evaluated; of them, rows whose 1/4 .. 4/4 prefix fails the bound
+  unsigned long long prof_vtest = 0, prof_migrated = 0;  // hash-set test-and-inserts of this thread; queries moved to the bitmap
 #else
   unsigned long long* prefix_cnt = nullptr;
 #endif
@@ -343,11 +375,19 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
     // ---- seed (InitializeSetLPara): precomputed distances of the query-independent seed set ----
     for (int i = tid; i < a.dim; i += kGsThreads) qv[i] = a.queries[static_cast<int64_t>(q) * a.dim + i];
     for (int i = a.dim + tid; i < dim4p; i += kGsThreads) qv[i] = 0.f;
+    bool hashed = L <= a.vset_max;  // the visited set is the hash set (false: the query has moved to the bitmap)
     for (int i = tid; i < a.Lp; i += kGsThreads) {
       unsigned long long key = kKeyInf;
       if (i < L) {
         const uint32_t id = static_cast<uint32_t>(a.init_ids[i]);
-        atomicOr(&visited[id >> 5], 1u << (id & 31));
+        if (hashed) {
+          vset_claim(vset, vmask, vset_bucket(id, a.vset_shift), id, vacc);
+#ifdef EPS_GS_PROFILE
+          ++prof_vtest;
+#endif
+        } else {
+          atomicOr(&visited[id >> 5], 1u << (id & 31));
+        }
         key = make_key(a.seed_dist[static_cast<int64_t>(q) * a.seed_ld + i], id);
       }
       qa[i] = key;
@@ -418,7 +458,9 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
               if (staged) {
                 const uint32_t bar = bar0 + 8 * slot;
                 mbar_expect_tx(bar, row_bytes);
-                bulk_load_1d(ring0 + slot * static_cast<uint32_t>(a.slot_bytes), a.vectors + static_cast<int64_t>(id) * a.dim, row_bytes, bar);
+                // rows are mostly read once: L2 evicts them first, so that they do not push out the visited tables
+                bulk_load_1d(ring0 + slot * static_cast<uint32_t>(a.slot_bytes), a.vectors + static_cast<int64_t>(id) * a.dim, row_bytes, bar,
+                             l2_policy_evict_first());
               }
             }
           }
@@ -526,6 +568,20 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
         e0 = s_cont_e[ncont - 1];
         nslots = static_cast<int>(min(static_cast<long long>(kGsThreads), s_cont_end[ncont - 1] - e0));
       }
+      // a step inserts at most nslots ids: move to the bitmap before the hash set could pass 3/4 full.  Every id the
+      // query has visited is a seed or in the log (fifo_tail <= vset_max < vlog_cap).  Block-uniform.
+      if (hashed && L + fifo_tail + static_cast<uint32_t>(nslots) > static_cast<uint32_t>(a.vset_max)) {
+        for (int i = tid; i < L; i += kGsThreads) {
+          const uint32_t id = static_cast<uint32_t>(a.init_ids[i]);
+          atomicOr(&visited[id >> 5], 1u << (id & 31));
+        }
+        for (uint32_t i = tid; i < fifo_tail; i += kGsThreads) {
+          const uint32_t id = static_cast<uint32_t>(vlog[i]);
+          atomicOr(&visited[id >> 5], 1u << (id & 31));
+        }
+        hashed = false;
+        __syncthreads();  // every bit is set before any thread tests one
+      }
       int nb[kRounds];
       unsigned bal[kRounds];
       bool fr[kRounds];
@@ -536,12 +592,52 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
         if (s < nslots)
           nb[r] = cont_mode ? a.nbrs[e0 + s] : __ldg(a.ell + static_cast<int64_t>(s_cid[s >> 6]) * kEll + (s & (kEll - 1)));
       }
+      // test-and-insert (ExpandOneCandidate :403-406); of two slots racing on one id exactly one finds it fresh
+      if (hashed) {
+        // one bucket read per id: an entry equal to it = visited; else a CAS on the first free entry of the bucket (the
+        // next bucket's first entry when it is full), and a CAS lost to another id goes on probing entry by entry
+        uint32_t at[kRounds], old[kRounds];
 #pragma unroll
-      for (int r = 0; r < kRounds; ++r) {
-        fr[r] = false;
-        if (nb[r] >= 0) {
-          const uint32_t bit = 1u << (nb[r] & 31);
-          fr[r] = !(atomicOr(&visited[nb[r] >> 5], bit) & bit);  // ExpandOneCandidate :403-406
+        for (int r = 0; r < kRounds; ++r) {
+          at[r] = kVsetEmpty;
+          if (nb[r] >= 0) {
+            const uint32_t id = static_cast<uint32_t>(nb[r]), b = vset_bucket(id, a.vset_shift);
+            const uint4 lo = __ldcg(reinterpret_cast<const uint4*>(vset + b)), hi = __ldcg(reinterpret_cast<const uint4*>(vset + b) + 1);
+            const uint32_t e[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+            bool hit = false;
+            uint32_t fe = 8;
+#pragma unroll
+            for (int j = 7; j >= 0; --j) {
+              hit |= e[j] == id;
+              if (e[j] == kVsetEmpty) fe = j;
+            }
+            if (!hit) at[r] = (b + fe) & vmask;
+#ifdef EPS_GS_PROFILE
+            ++prof_vtest; ++vacc;
+#endif
+          }
+        }
+#pragma unroll
+        for (int r = 0; r < kRounds; ++r) old[r] = at[r] != kVsetEmpty ? atomicCAS(vset + at[r], kVsetEmpty, static_cast<uint32_t>(nb[r])) : 0u;
+#pragma unroll
+        for (int r = 0; r < kRounds; ++r) {
+          fr[r] = false;
+          if (at[r] != kVsetEmpty) {
+#ifdef EPS_GS_PROFILE
+            ++vacc;
+#endif
+            const uint32_t id = static_cast<uint32_t>(nb[r]);
+            fr[r] = old[r] == kVsetEmpty || (old[r] != id && vset_claim(vset, vmask, (at[r] + 1) & vmask, id, vacc));
+          }
+        }
+      } else {
+#pragma unroll
+        for (int r = 0; r < kRounds; ++r) {
+          fr[r] = false;
+          if (nb[r] >= 0) {
+            const uint32_t bit = 1u << (nb[r] & 31);
+            fr[r] = !(atomicOr(&visited[nb[r] >> 5], bit) & bit);
+          }
         }
       }
 #pragma unroll
@@ -610,6 +706,16 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
       a.qtimes[4 * q + 1] = t; a.qtimes[4 * q + 2] = st_ndist - prof_nd0; a.qtimes[4 * q + 3] = prof_iters;
     }
 #endif
+    // the hash set: 16-byte stores over the whole table (at most 64 KB, in L2); the bitmap only if the query moved to it
+    {
+      uint4* t4 = reinterpret_cast<uint4*>(vset);
+      const uint4 e = make_uint4(kVsetEmpty, kVsetEmpty, kVsetEmpty, kVsetEmpty);
+      for (int i = tid; i < (a.vset_cap >> 2); i += kGsThreads) t4[i] = e;
+    }
+#ifdef EPS_GS_PROFILE
+    if (tid == 0 && !hashed) ++prof_migrated;
+#endif
+    if (hashed) continue;
     if (fifo_tail <= static_cast<uint32_t>(a.vlog_cap) && 10ll * (fifo_tail + L) < a.visited_words) {
       // large table: clear only the words this query touched (the seeds and the logged fresh ids) instead of
       // streaming zeros over the whole bitmap (1.25 MB per query at 10M rows)
@@ -628,6 +734,9 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
     if (warp == 0) atomicAdd(&a.stats[24], static_cast<unsigned long long>(clock64() - t_kernel0));
   }
   for (int i = 0; i < 5; ++i) if (prefix_cnt[i]) atomicAdd(&a.stats[25 + i], prefix_cnt[i]);
+  if (prof_vtest) atomicAdd(&a.stats[5], prof_vtest);
+  if (prof_migrated) atomicAdd(&a.stats[30], prof_migrated);
+  if (vacc) atomicAdd(&a.stats[31], vacc);
 #endif
   if (st_ndist) atomicAdd(&a.stats[0], st_ndist);
   if (st_nexp) atomicAdd(&a.stats[1], st_nexp);
@@ -782,7 +891,19 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
     ix->vis_clean_words = words;
     ix->vis_clean_cap = ix->s_visited.cap;
   }
-  EPS_TRY(ix->s_misc.reserve(256));  // [0..3] counters, [+32 B] work counter, [8..24] developer phase timers, [25..29] developer prefix counts
+  // Visited hash sets: 16 entries per queue slot, so that the ~10 L ids a query visits load its table about 2/3 (a
+  // query that needs more moves to its bitmap), and at most 16384 entries = 64 KB per slot: the tables of the 528
+  // queries resident at the benchmark's geometry take 34 MB of the 50 MB L2.  The kernel refills every table it
+  // touched, so the whole buffer is all-ones between launches whatever the table size; fill it when it is (re)allocated.
+  const int vset_cap = std::min(16384, std::max(1024, next_pow2(16 * static_cast<int>(L))));
+  EPS_TRY(ix->s_vset.reserve(static_cast<size_t>(slots) * vset_cap * 4));
+  if (ix->vset_clean_ptr != ix->s_vset.p || ix->vset_clean_cap != ix->s_vset.cap) {
+    EPS_CUDA(cudaMemsetAsync(ix->s_vset.p, 0xff, ix->s_vset.cap, ix->stream));
+    ix->vset_clean_ptr = ix->s_vset.p;
+    ix->vset_clean_cap = ix->s_vset.cap;
+  }
+  EPS_TRY(ix->s_misc.reserve(256));  // [0..3] counters, [+32 B] work counter, [5] [30..31] developer hash-set counts,
+                                     // [8..24] developer phase timers, [25..29] developer prefix counts
   EPS_CUDA(cudaMemsetAsync(ix->s_misc.p, 0, 256, ix->stream));
   uint64_t launches = 1;
   EPS_TRY(ensure_ell(ix, &launches));
@@ -805,6 +926,8 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   constexpr int kVlogCap = 32768;
   EPS_TRY(ix->s_vlog.reserve(static_cast<size_t>(slots) * kVlogCap * 4));
   a.vlog = ix->s_vlog.as<int32_t>(); a.vlog_cap = kVlogCap;
+  a.vset = ix->s_vset.as<uint32_t>(); a.vset_cap = vset_cap; a.vset_max = vset_cap / 4 * 3;
+  a.vset_shift = 32 - (__builtin_ctz(static_cast<unsigned>(vset_cap)) - 3);
   a.visited = ix->s_visited.as<uint32_t>(); a.out_queue = d_queue;
   a.work_counter = reinterpret_cast<int*>(ix->s_misc.as<unsigned char>() + 32);
   a.stats = ix->s_misc.as<unsigned long long>();
@@ -847,6 +970,10 @@ int read_graph_counters(Index* ix, eps_stats* stats) {
   for (int w = 0; w < 2; ++w)
     for (int i = 0; i < 8; ++i) fprintf(stderr, " w%d.%s=%.1f%%", w, names[i], 100.0 * static_cast<double>(pr[8 + w * 8 + i]) / tot);
   fprintf(stderr, "\n");
+  fprintf(stderr, "[gs-profile] visited hash set: %llu test-and-inserts, %.3f table accesses (bucket reads + CAS) each; "
+                  "%llu queries moved to the bitmap (%.2f%%)\n",
+          pr[5], static_cast<double>(pr[31]) / (static_cast<double>(pr[5]) + 1e-9), pr[30],
+          ix->prof_nq > 0 ? 100.0 * static_cast<double>(pr[30]) / static_cast<double>(ix->prof_nq) : 0.0);
   if (pr[25]) {
     // fetching a prefix s of every row and the rest only where the prefix cannot reject it would stage
     // s + (1 - p(s)) (1 - s) of the row bytes, p(s) = share of rows whose prefix s fails the bound

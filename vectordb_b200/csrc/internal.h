@@ -82,7 +82,7 @@ struct Index {
   int num_sms = 132;
 
   // scratch
-  DevBuf s_queries, s_dist, s_topk, s_topk2, s_pass, s_filter, s_visited, s_vlog, s_queue, s_tail, s_out_ids, s_out_dists,
+  DevBuf s_queries, s_dist, s_topk, s_topk2, s_pass, s_filter, s_vset, s_visited, s_vlog, s_queue, s_tail, s_out_ids, s_out_dists,
       s_out_counts, s_stats, s_misc, s_seed_rows, s_seed_dist, s_xnorm, s_qnorm, s_coarse, s_thr, s_cand, s_cand_cnt, s_bf16, s_qbf16, s_flags;
   int coarse_mode = 1;           // exact-scan coarse pass: 0 = fp32 SIMT only, 1 = wgmma TF32, 2 = wgmma bf16 mirror
   int coarse_guard = 1;          // verify the coarse pass after the re-score and redo unsafe queries (brute_force.cu)
@@ -95,6 +95,8 @@ struct Index {
   const void* vis_clean_ptr = nullptr;  // geometry for which the visited bitmaps are known to be zero
   int64_t vis_clean_words = 0;
   size_t vis_clean_cap = 0;
+  const void* vset_clean_ptr = nullptr;  // visited hash-set buffer known to be all-ones (empty), and its capacity
+  size_t vset_clean_cap = 0;
   bool graph_counters_pending = false;
   int64_t prof_nq = 0;           // developer build (EPS_GS_PROFILE): queries of the last profiled launch
   void* h_out = nullptr;         // pinned host mirror of the packed result block (eps_search_batch)

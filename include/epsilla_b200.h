@@ -262,6 +262,46 @@ EPS_API int eps_normalize(int device, float* host_vectors, int64_t nq, int64_t d
 EPS_API int eps_pair_distances(int device, int metric, const float* a, const float* b, int64_t n_pairs, int64_t dim,
                        float* out);
 
+/* ---------------------------------------------------------------------------------------------
+ * Sparse-vector fields (SPARSE_VECTOR_FLOAT / _DOUBLE, db/vector.hpp:13-20): TableSegmentMVP::var_len_attr_table_
+ * rows of {index, value} pairs mirrored as a device CSR (int64 row offsets, interleaved {uint32 index, float value}
+ * elements, one fp32 |row|^2 per row for cosine).
+ *
+ * These calls work on a sparse index as on a dense one: eps_index_set_deleted, eps_index_set_attrs,
+ * eps_index_set_string_codes, eps_index_config, eps_index_create_view (the view shares the CSR), eps_index_build,
+ * eps_index_get_graph, eps_index_rows, eps_facet_batch.  The dense-only calls (sync_rows, adopt_device_rows,
+ * device_rows, set_graph, set_coarse, set_search_width, set_graph_tuning, eps_search_batch*,
+ * eps_search_batch_sharded) fail with EPS_ERR_INVALID_ARGUMENT (device_rows returns NULL).
+ * --------------------------------------------------------------------------------------------- */
+
+/* dim = the field's vector_dimension_ (< 2^32 - 1): every index of a row is < dim (table_segment_mvp.cpp:525-533).
+ * capacity_rows is a hint; the mirror grows as rows are appended. */
+EPS_API int eps_index_create_sparse(eps_index** out, int metric, int64_t dim, int64_t capacity_rows, int device);
+
+/* Append rows [first_row, first_row + n_rows); first_row must equal the rows already mirrored.  Row r is
+ * indices / values [offsets[r], offsets[r+1]) (offsets[0] need not be 0).  Rows with a negative index, an index
+ * >= dim, or indices that are not strictly increasing are rejected with EPS_ERR_INVALID_ARGUMENT, as the reference's
+ * insert rejects them (table_segment_mvp.cpp:539-550); nothing is appended then.  Empty rows are legal.  Values are
+ * stored as given (the reference normalises cosine rows at insert, :556-562). */
+EPS_API int eps_index_append_sparse_rows(eps_index* ix, int64_t first_row, int64_t n_rows, const int64_t* offsets,
+                                         const int64_t* indices, const float* values);
+
+/* VecSearchExecutor::Search of nq sparse queries (CSR like the rows; indices strictly increasing, < 2^32 - 1), with the
+ * output contract of eps_search_batch.  Distances are bit-identical to GetL2DistSqr / GetInnerProductDist /
+ * GetCosineDist (db/vector.cpp:7-100, row = v1, query = v2): the same sequential fp32 sums in the same order, no FMA.
+ * Cosine queries must already be normalised (db/table_mvp.cpp:337-349), like dense ones.
+ * A sparse index ALWAYS answers by the exact scan over all mirrored rows, with the reference's brute-force caps
+ * (prefilter / force_brute: limit results; otherwise min(limit, L_local)), even when a graph is installed.  This is
+ * the one deliberate deviation from the reference: where it would search its graph (n_indexed >= 512), the GPU returns
+ * the exact top-k.  Cosine with an empty row or an empty query gives 0/0 = NaN (the reference's std::sort order of
+ * such entries is unspecified): NaN distances sort after every number.  eps_stats.n_dist counts nq x the rows scanned.
+ * eps_index_build on a sparse index installs the exact out_degree-NN lists (field metric, self excluded), the L2
+ * nearest row to the reference's sparse centre (nsg.cpp:120-135) as navigation point, and repair edges that make every
+ * row reachable from it.  HOST buffers in and out. */
+EPS_API int eps_search_sparse_batch(eps_index* ix, int64_t nq, const int64_t* q_offsets, const int64_t* q_indices,
+                                    const float* q_values, int64_t limit, const eps_filter_node* filter, int64_t n_filter,
+                                    int64_t* out_ids, double* out_dists, int64_t* out_counts, eps_stats* stats);
+
 /* Raw stream handle (cudaStream_t) the index launches on, for callers that time with CUDA events. */
 EPS_API void* eps_index_stream(eps_index* ix);
 

@@ -3,9 +3,9 @@
 The product is ``libepsilla_b200.so`` (hand-written CUDA, ``csrc/``) declared in
 ``include/epsilla_b200.h``.  This package is the thin Python host layer used by the tests and
 ``bench.py``: a ctypes loader that FAILS LOUDLY when the library is missing (there is no CPU
-fallback) and an ``Index`` class that mirrors the C ABI one-to-one.
+fallback) and an ``Index`` class (and ``SparseIndex`` for sparse-vector fields) that mirrors the C ABI one-to-one.
 """
 from .lib import load_library, library_path, EpsError  # noqa: F401
-from .index import Index, Stats, METRICS, filter_nodes_array  # noqa: F401
+from .index import Index, SparseIndex, Stats, METRICS, filter_nodes_array  # noqa: F401
 
-__all__ = ["load_library", "library_path", "EpsError", "Index", "Stats", "METRICS", "filter_nodes_array"]
+__all__ = ["load_library", "library_path", "EpsError", "Index", "SparseIndex", "Stats", "METRICS", "filter_nodes_array"]

@@ -483,7 +483,8 @@ int launch_distances(Index* ix, const float* A_base, int64_t row_start, int64_t 
 
 static int topk_impl(Index* ix, const float* d_queries, int64_t nq, int64_t row_start, int64_t row_end, int64_t k,
                      const FilterProg* d_prog, const FilterProg* h_prog, bool prefilter, int64_t self_base,
-                     unsigned long long* d_topk, eps_stats* stats, bool allow_tc = true) {
+                     unsigned long long* d_topk, eps_stats* stats, bool allow_tc = true,
+                     const DistProducer* producer = nullptr) {
   // never-shrinking scratch owned by the index would be overwritten by the nested fp32 redo of unsafe queries
   // (that redo never takes the tensor-core branch, so it uses none of the coarse-pass buffers)
   if (k < 1 || k > 8192) return fail(EPS_ERR_UNSUPPORTED, "brute-force top-k supports 1 <= k <= 8192");
@@ -494,7 +495,7 @@ static int topk_impl(Index* ix, const float* d_queries, int64_t nq, int64_t row_
   const bool dyn_filter = h_prog && h_prog->n > 0 && !prefilter && h_prog->root_uses_dist;
   const int64_t k_final = k;
   unsigned long long* d_final = d_topk;
-  const bool use_tc = allow_tc && n >= 4096 && self_base < 0 && !dyn_filter && tc_dist_usable(ix, nq) && d_queries != ix->d_vectors;
+  const bool use_tc = !producer && allow_tc && n >= 4096 && self_base < 0 && !dyn_filter && tc_dist_usable(ix, nq) && d_queries != ix->d_vectors;
   if (use_tc) {
     // k' coarse candidates per query: k + max(118, k) (128 for top-10), times the boost the guard has learnt
     static const int64_t env_kmin = [] { const char* e = getenv("EPS_SCAN_KMIN"); return e ? atoll(e) : 118ll; }();  // developer knob
@@ -598,6 +599,7 @@ static int topk_impl(Index* ix, const float* d_queries, int64_t nq, int64_t row_
     a.thr_out = use_tc ? ix->s_thr.as<float>() : nullptr;
     if (!fused) {
       if (use_tc) EPS_TRY(tc_launch_distances(ix, row_start + c0, cn, d_queries, nq, D, chunk, &launches));
+      else if (producer) EPS_TRY(producer->launch(ix, row_start + c0, cn, D, chunk, &launches));
       else EPS_TRY(launch_distances(ix, ix->d_vectors, row_start + c0, cn, d_queries, nq, D, chunk, &launches));
       a.D = D; a.keys_in = nullptr; a.n = cn;
       TL_MARK("dist tile " + std::to_string(cn));
@@ -729,6 +731,12 @@ int brute_force_topk(Index* ix, const float* d_queries, int64_t nq, int64_t row_
     return EPS_OK;
   }
   return topk_impl(ix, d_queries, nq, row_start, row_end, k, d_prog, h_prog, prefilter, -1, d_topk, stats);
+}
+
+int scan_topk(Index* ix, const DistProducer& dist, int64_t nq, int64_t row_start, int64_t row_end, int64_t k,
+              const FilterProg* d_prog, const FilterProg* h_prog, bool prefilter, int64_t self_base,
+              unsigned long long* d_topk, eps_stats* stats) {
+  return topk_impl(ix, nullptr, nq, row_start, row_end, k, d_prog, h_prog, prefilter, self_base, d_topk, stats, false, &dist);
 }
 
 int brute_force_knn_rows(Index* ix, int64_t q_start, int64_t nq, int64_t n_rows, int64_t k,

@@ -210,8 +210,7 @@ static int prune_pass(Index* ix, int64_t n, const unsigned long long* d_knn, int
   return EPS_OK;
 }
 
-// Install a host CSR (int64 offsets, int32 ids) as the index's graph, dropping everything derived from the old one.
-static int install_csr(Index* ix, int64_t n, const int64_t* off, const int32_t* nb, int64_t e, int64_t nav) {
+int install_csr(Index* ix, int64_t n, const int64_t* off, const int32_t* nb, int64_t e, int64_t nav) {
   if (ix->d_offsets) { cudaFree(ix->d_offsets); ix->d_offsets = nullptr; }
   if (ix->d_nbrs) { cudaFree(ix->d_nbrs); ix->d_nbrs = nullptr; }
   if (ix->d_init_ids) { cudaFree(ix->d_init_ids); ix->d_init_ids = nullptr; }
@@ -228,6 +227,76 @@ static int install_csr(Index* ix, int64_t n, const int64_t* off, const int32_t* 
   ix->n_edges = e;
   ix->nav = nav;
   return EPS_OK;
+}
+
+ConnRepair::ConnRepair(int64_t n_, const int32_t* lists_, const int32_t* cnt_, int stride_)
+    : n(n_), lists(lists_), cnt(cnt_), stride(stride_), seen(static_cast<size_t>(n_), 0), extra(static_cast<size_t>(n_)) {}
+
+void ConnRepair::flood(int32_t root) {
+  if (seen[root]) return;
+  seen[root] = 1; ++linked;
+  stack.push_back(root);
+  while (!stack.empty()) {
+    const int32_t u = stack.back();
+    stack.pop_back();
+    const int32_t* row = &lists[static_cast<size_t>(u) * stride];
+    for (int j = 0; j < cnt[u]; ++j) {
+      const int32_t w = row[j];
+      if (!seen[w]) { seen[w] = 1; ++linked; stack.push_back(w); }
+    }
+    for (int32_t w : extra[u]) if (!seen[w]) { seen[w] = 1; ++linked; stack.push_back(w); }
+  }
+}
+
+void ConnRepair::attach_from_knn(const unsigned long long* knn, int K) {
+  constexpr size_t kRepairCap = 16;
+  for (int64_t u = 0; u < n && linked < n; ++u) {
+    if (seen[u]) continue;
+    bool any_linked = false, done = false;
+    for (int j = 0; j < K && !done; ++j) {  // 1. nearest linked kNN entry with room
+      const unsigned long long key = knn[static_cast<size_t>(u) * K + j];
+      if ((key & kKeyMask) == kKeyInf) break;
+      const int32_t w = static_cast<int32_t>(key_id(key));
+      if (!seen[w]) continue;
+      any_linked = true;
+      if (extra[w].size() < kRepairCap) {
+        extra[w].push_back(static_cast<int32_t>(u));
+        flood(static_cast<int32_t>(u));
+        done = true;
+      }
+    }
+    if (!done && !any_linked) {  // 2. a component of its own: u is its entry (wired up in flatten)
+      entries.push_back(static_cast<int32_t>(u));
+      flood(static_cast<int32_t>(u));
+    }
+  }
+}
+
+void ConnRepair::attach_random(int32_t u, uint64_t* rng) {
+  int32_t root = -1;
+  while (root < 0) {  // a random linked vertex (:767-774)
+    *rng = *rng * 6364136223846793005ull + 1442695040888963407ull;
+    const int32_t r = static_cast<int32_t>((*rng >> 33) % static_cast<uint64_t>(n));
+    if (seen[r]) root = r;
+  }
+  extra[root].push_back(u);  // nsg[root].push_back(id) (:774), may exceed out_degree (Q11)
+  flood(u);
+}
+
+void ConnRepair::flatten(int64_t nav, std::vector<int64_t>* off, std::vector<int32_t>* nb) {
+  // entries of the separate components: out-neighbours of the navigation point
+  for (int32_t u : entries) extra[nav].push_back(u);
+  entries.clear();
+  off->assign(static_cast<size_t>(n) + 1, 0);
+  int64_t e = 0;
+  for (int64_t v = 0; v < n; ++v) { (*off)[v] = e; e += cnt[v] + static_cast<int64_t>(extra[v].size()); }
+  (*off)[n] = e;
+  nb->assign(static_cast<size_t>(e), 0);
+  for (int64_t v = 0; v < n; ++v) {
+    int64_t o = (*off)[v];
+    for (int j = 0; j < cnt[v]; ++j) (*nb)[o++] = lists[static_cast<size_t>(v) * stride + j];
+    for (int32_t w : extra[v]) (*nb)[o++] = w;
+  }
 }
 
 int build_graph(Index* ix, int64_t n, const eps_build_params* params) {
@@ -352,50 +421,12 @@ int build_graph(Index* ix, int64_t n, const eps_build_params* params) {
   //      through graph_search on the device (L2 like the rest of the refinement, beam = max(64, search_length));
   //   4. a random linked vertex (:767-774).
   // The attach / flood bookkeeping — integer work — runs on the host in the reference's order.
-  constexpr size_t kRepairCap = 16;
-  std::vector<int32_t> entries;  // one per component that the kNN lists do not connect to the rest
-  std::vector<std::vector<int32_t>> extra(static_cast<size_t>(n));  // edges added by the repair
+  ConnRepair rep(n, h_ids.data(), h_cnt.data(), stride);
   {
-    std::vector<uint8_t> seen(static_cast<size_t>(n), 0);
-    std::vector<int32_t> stack;
-    int64_t linked = 0;
-    auto flood = [&](int32_t root) {
-      if (seen[root]) return;
-      seen[root] = 1; ++linked;
-      stack.push_back(root);
-      while (!stack.empty()) {
-        const int32_t u = stack.back();
-        stack.pop_back();
-        const int32_t* row = &h_ids[static_cast<size_t>(u) * stride];
-        for (int j = 0; j < h_cnt[u]; ++j) {
-          const int32_t w = row[j];
-          if (!seen[w]) { seen[w] = 1; ++linked; stack.push_back(w); }
-        }
-        for (int32_t w : extra[u]) if (!seen[w]) { seen[w] = 1; ++linked; stack.push_back(w); }
-      }
-    };
-    flood(static_cast<int32_t>(nav));
-    for (int64_t u = 0; u < n && linked < n; ++u) {
-      if (seen[u]) continue;
-      bool any_linked = false, done = false;
-      for (int j = 0; j < K && !done; ++j) {  // 1. nearest linked kNN entry with room
-        const unsigned long long key = h_knn[static_cast<size_t>(u) * K + j];
-        if ((key & kKeyMask) == kKeyInf) break;
-        const int32_t w = static_cast<int32_t>(key_id(key));
-        if (!seen[w]) continue;
-        any_linked = true;
-        if (extra[w].size() < kRepairCap) {
-          extra[w].push_back(static_cast<int32_t>(u));
-          flood(static_cast<int32_t>(u));
-          done = true;
-        }
-      }
-      if (!done && !any_linked) {  // 2. a component of its own: u is its entry (wired up below)
-        entries.push_back(static_cast<int32_t>(u));
-        flood(static_cast<int32_t>(u));
-      }
-    }
-    if (linked < n) {
+    rep.flood(static_cast<int32_t>(nav));
+    rep.attach_from_knn(h_knn.data(), K);  // steps 1 and 2
+    std::vector<uint8_t>& seen = rep.seen;
+    if (rep.linked < n) {
       std::vector<int32_t> unl;
       for (int64_t v = 0; v < n; ++v) if (!seen[v]) unl.push_back(static_cast<int32_t>(v));
       // install the un-repaired graph for the batched searches
@@ -441,37 +472,24 @@ int build_graph(Index* ix, int64_t n, const eps_build_params* params) {
           if (seen[u]) continue;  // reached through an earlier attachment of this chunk
           int32_t root = -1;
           const unsigned long long* pool = &h_pool[static_cast<size_t>(i) * Ls];
-          for (int64_t j = 0; j < Ls; ++j) {  // nearest linked vertex of the search pool (:757-766)
+          for (int64_t j = 0; j < Ls; ++j) {  // 3. nearest linked vertex of the search pool (:757-766)
             if ((pool[j] & kKeyMask) == kKeyInf) break;
             const int32_t w = static_cast<int32_t>(key_id(pool[j]));
             if (w != u && seen[w]) { root = w; break; }
           }
-          while (root < 0) {  // a random linked vertex (:767-774)
-            rng = rng * 6364136223846793005ull + 1442695040888963407ull;
-            const int32_t r = static_cast<int32_t>((rng >> 33) % static_cast<uint64_t>(n));
-            if (seen[r]) root = r;
-          }
-          extra[root].push_back(u);  // nsg[root].push_back(id) (:774), may exceed out_degree (Q11)
-          flood(u);
+          if (root < 0) { rep.attach_random(u, &rng); continue; }  // 4.
+          rep.extra[root].push_back(u);  // nsg[root].push_back(id) (:774), may exceed out_degree (Q11)
+          rep.flood(u);
         }
       }
       ix->graph_counters_pending = false;
       if (rc != EPS_OK) return rc;
     }
   }
-  // ---- entries of the separate components: out-neighbours of the navigation point ----
-  for (int32_t u : entries) extra[nav].push_back(u);
-
-  std::vector<int64_t> off(static_cast<size_t>(n) + 1);
-  int64_t e = 0;
-  for (int64_t v = 0; v < n; ++v) { off[v] = e; e += h_cnt[v] + static_cast<int64_t>(extra[v].size()); }
-  off[n] = e;
-  std::vector<int32_t> nb(static_cast<size_t>(e));
-  for (int64_t v = 0; v < n; ++v) {
-    int64_t o = off[v];
-    for (int j = 0; j < h_cnt[v]; ++j) nb[o++] = h_ids[static_cast<size_t>(v) * stride + j];
-    for (int32_t w : extra[v]) nb[o++] = w;
-  }
+  std::vector<int64_t> off;
+  std::vector<int32_t> nb;
+  rep.flatten(nav, &off, &nb);
+  const int64_t e = off[n];
   EPS_TRY(install_csr(ix, n, off.data(), nb.data(), e, nav));
   return EPS_OK;
 }

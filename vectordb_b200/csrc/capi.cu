@@ -248,6 +248,49 @@ static int search_device(Index* ix, const float* d_queries, int64_t nq, int64_t 
   return EPS_OK;
 }
 
+// search_device for a sparse index: always the exact scan over [0, total) with the brute-force branch's caps
+// (:857 prefilter: limit; :864 brute: min(limit, L_local)), whatever graph is installed.
+static int search_sparse_device(Index* ix, const SparseQueries& q, int64_t nq, int64_t limit, const eps_filter_node* filter,
+                                int64_t n_filter, int64_t* d_ids, float* d_dists, int64_t* d_counts, eps_stats* stats) {
+  if (nq <= 0) return EPS_OK;
+  FilterProg h_prog;
+  EPS_TRY(lower_filter(filter, n_filter, &h_prog));
+  const FilterProg* d_prog = nullptr;
+  if (h_prog.n > 0) {
+    EPS_TRY(bind_program_columns(ix, &h_prog));
+    EPS_TRY(ix->s_filter.reserve(sizeof(FilterProg)));
+    EPS_CUDA(cudaMemcpyAsync(ix->s_filter.p, &h_prog, sizeof(FilterProg), cudaMemcpyHostToDevice, ix->stream));
+    d_prog = ix->s_filter.as<FilterProg>();
+  }
+  const int64_t total = ix->n_rows;
+  const int64_t cap = (ix->prefilter || ix->force_brute) ? limit : std::min<int64_t>(limit, ix->L_local);
+  const int64_t k = std::max<int64_t>(1, std::min<int64_t>(cap, total));
+  if (k > 8192) return fail(EPS_ERR_UNSUPPORTED, "more than 8192 results per query from the exact scan are not supported");
+  eps_stats local;
+  std::memset(&local, 0, sizeof(local));
+  if (stats) EPS_CUDA(cudaEventRecord(ix->ev[1], ix->stream));
+  EPS_TRY(ix->s_topk.reserve(static_cast<size_t>(nq) * k * 8));
+  SparseDist dist;
+  dist.q = q;
+  dist.nq = nq;
+  dist.metric = ix->metric;
+  EPS_TRY(scan_topk(ix, dist, nq, 0, total, k, d_prog, &h_prog, ix->prefilter, -1, ix->s_topk.as<unsigned long long>(), &local));
+  if (stats) EPS_CUDA(cudaEventRecord(ix->ev[2], ix->stream));
+  EPS_TRY(finalize_keys(ix, ix->s_topk.as<unsigned long long>(), nq, k, limit, cap, d_ids, d_dists, d_counts));
+  local.kernel_launches += 1;
+  if (stats) {
+    stats->n_dist += local.n_dist;
+    stats->n_queries += static_cast<uint64_t>(nq);
+    stats->kernel_launches += local.kernel_launches;
+  }
+  return EPS_OK;
+}
+
+static int dense_only(const Index* ix) {
+  if (ix->sparse) return fail(EPS_ERR_INVALID_ARGUMENT, "dense-vector call on a sparse index");
+  return EPS_OK;
+}
+
 }  // namespace eps
 
 using eps::Index;
@@ -295,6 +338,31 @@ int eps_index_create(eps_index** out, int metric, int64_t dim, const float* host
   return EPS_OK;
 }
 
+int eps_index_create_sparse(eps_index** out, int metric, int64_t dim, int64_t capacity_rows, int device) {
+  if (!out) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "out is null");
+  *out = nullptr;
+  if (dim < 1 || dim >= 0xffffffffll || capacity_rows < 0)
+    return eps::fail(EPS_ERR_INVALID_ARGUMENT, "bad dim (must be in [1, 2^32 - 1)) / capacity");
+  if (metric != EPS_METRIC_L2 && metric != EPS_METRIC_COSINE && metric != EPS_METRIC_IP) metric = EPS_METRIC_L2;
+  EPS_TRY(eps::check_device(device));
+  eps_index* h = nullptr;
+  EPS_TRY(eps_index_create(&h, metric, dim, nullptr, 0, device));
+  Index* ix = reinterpret_cast<Index*>(h);
+  ix->sparse = true;
+  ix->capacity = capacity_rows;
+  const int64_t rows = std::max<int64_t>(capacity_rows, 1);
+  cudaError_t e = cudaMalloc(&ix->d_sp_ptr, static_cast<size_t>(rows + 1) * 8);
+  if (e == cudaSuccess) e = cudaMalloc(&ix->d_sp_norm2, static_cast<size_t>(rows) * 4);
+  if (e == cudaSuccess) e = cudaMemset(ix->d_sp_ptr, 0, 8);
+  if (e != cudaSuccess) {
+    eps_index_destroy(h);
+    return eps::fail(EPS_ERR_OOM, std::string("sparse row table: ") + cudaGetErrorString(e));
+  }
+  ix->sp_row_cap = rows;
+  *out = h;
+  return EPS_OK;
+}
+
 void eps_index_destroy(eps_index* h) {
   if (!h) return;
   Index* ix = reinterpret_cast<Index*>(h);
@@ -315,6 +383,7 @@ void eps_index_destroy(eps_index* h) {
       v->d_offsets = nullptr; v->d_nbrs = nullptr; v->d_ell = nullptr; v->n_indexed = 0; v->n_edges = 0;
       v->d_deleted = nullptr; v->deleted_bytes = 0; v->any_deleted = false;
       v->d_attrs = nullptr; v->attr_rows = 0;
+      v->d_sp_ptr = nullptr; v->d_sp_elems = nullptr; v->d_sp_norm2 = nullptr; v->sp_nnz = 0;
       for (auto& sc : v->str_cols) sc = eps::StrCol();
     }
     ix->views.clear();
@@ -323,10 +392,13 @@ void eps_index_destroy(eps_index* h) {
     if (ix->d_deleted) cudaFree(ix->d_deleted);
     if (ix->d_attrs) cudaFree(ix->d_attrs);
     for (auto& sc : ix->str_cols) if (sc.d_codes) cudaFree(sc.d_codes);
+    if (ix->d_sp_ptr) cudaFree(ix->d_sp_ptr);
+    if (ix->d_sp_elems) cudaFree(ix->d_sp_elems);
+    if (ix->d_sp_norm2) cudaFree(ix->d_sp_norm2);
   }
   eps::DevBuf* bufs[] = {&ix->s_queries, &ix->s_dist, &ix->s_topk, &ix->s_topk2, &ix->s_pass, &ix->s_filter,
                          &ix->s_vset, &ix->s_visited, &ix->s_vlog, &ix->s_queue, &ix->s_tail, &ix->s_out_ids, &ix->s_out_dists,
-                         &ix->s_out_counts, &ix->s_stats, &ix->s_misc, &ix->s_seed_rows, &ix->s_seed_dist, &ix->s_xnorm, &ix->s_qnorm, &ix->s_coarse, &ix->s_thr, &ix->s_cand, &ix->s_cand_cnt, &ix->s_bf16, &ix->s_qbf16, &ix->s_flags};
+                         &ix->s_out_counts, &ix->s_stats, &ix->s_misc, &ix->s_seed_rows, &ix->s_seed_dist, &ix->s_xnorm, &ix->s_qnorm, &ix->s_coarse, &ix->s_thr, &ix->s_cand, &ix->s_cand_cnt, &ix->s_bf16, &ix->s_qbf16, &ix->s_flags, &ix->s_sparse_q};
   for (auto* b : bufs) b->release();
   if (ix->h_out) cudaFreeHost(ix->h_out);
   for (auto& ev : ix->ev) if (ev) cudaEventDestroy(ev);
@@ -351,6 +423,8 @@ int eps_index_create_view(eps_index* base_h, eps_index** out) {
   ix->device = base->device; ix->metric = base->metric; ix->dim = base->dim; ix->capacity = base->capacity;
   ix->host_vectors = nullptr; ix->d_vectors = base->d_vectors; ix->owns_vectors = false; ix->n_rows = base->n_rows;
   ix->vec4 = base->vec4;
+  ix->sparse = base->sparse; ix->d_sp_ptr = base->d_sp_ptr; ix->d_sp_elems = base->d_sp_elems; ix->d_sp_norm2 = base->d_sp_norm2;
+  ix->sp_nnz = base->sp_nnz; ix->sp_elem_cap = base->sp_elem_cap; ix->sp_row_cap = base->sp_row_cap;
   ix->n_indexed = base->n_indexed; ix->n_edges = base->n_edges; ix->nav = base->nav;
   ix->d_offsets = base->d_offsets; ix->d_nbrs = base->d_nbrs; ix->d_ell = base->d_ell;
   ix->d_deleted = base->d_deleted; ix->deleted_bytes = base->deleted_bytes; ix->deleted_cap = base->deleted_cap;
@@ -382,6 +456,7 @@ int eps_index_sync_rows(eps_index* h, int64_t n_rows_now) {
   Index* ix = reinterpret_cast<Index*>(h);
   if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");
   EPS_TRY(eps::check_device(ix->device));
+  EPS_TRY(eps::dense_only(ix));
   EPS_TRY(check_mutable(ix));
   if (!ix->owns_vectors) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "index has no host vector table to mirror");
   if (n_rows_now < ix->n_rows || n_rows_now > ix->capacity)
@@ -399,6 +474,7 @@ int eps_index_sync_rows(eps_index* h, int64_t n_rows_now) {
 int eps_index_adopt_device_rows(eps_index* h, const float* d_vectors, int64_t n_rows) {
   Index* ix = reinterpret_cast<Index*>(h);
   if (!ix || !d_vectors) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null argument");
+  EPS_TRY(eps::dense_only(ix));
   EPS_TRY(eps::check_device(ix->device));
   EPS_TRY(check_mutable(ix));
   if (n_rows < 0 || n_rows >= (1ll << 31)) return eps::fail(EPS_ERR_UNSUPPORTED, "row count must be in [0, 2^31): keys carry 31-bit ids");
@@ -419,6 +495,7 @@ int eps_index_adopt_device_rows(eps_index* h, const float* d_vectors, int64_t n_
 int eps_index_set_graph(eps_index* h, int64_t n_indexed, const int64_t* offsets, const int64_t* nbrs, int64_t nav) {
   Index* ix = reinterpret_cast<Index*>(h);
   if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");
+  EPS_TRY(eps::dense_only(ix));
   EPS_TRY(eps::check_device(ix->device));
   EPS_TRY(check_mutable(ix));
   eps::free_graph(ix);
@@ -466,6 +543,7 @@ int eps_index_build(eps_index* h, int64_t n, const eps_build_params* params) {
   if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");
   EPS_TRY(eps::check_device(ix->device));
   EPS_TRY(check_mutable(ix));
+  if (ix->sparse) return eps::build_graph_sparse(ix, n, params);
   return eps::build_graph(ix, n, params);
 }
 
@@ -614,6 +692,7 @@ int eps_search_batch_device(eps_index* h, const float* d_queries, int64_t nq, in
   Index* ix = reinterpret_cast<Index*>(h);
   if (!ix || !d_queries || !d_out_ids || !d_out_dists || !d_out_counts)
     return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null argument");
+  EPS_TRY(eps::dense_only(ix));
   if (nq <= 0) return EPS_OK;  // nothing launched: no events to read back
   EPS_TRY(eps::check_device(ix->device));
   if (stats) EPS_CUDA(cudaEventRecord(ix->ev[0], ix->stream));
@@ -638,6 +717,7 @@ int eps_search_batch(eps_index* h, const float* queries, int64_t nq, int64_t lim
                      int64_t n_filter, int64_t* out_ids, double* out_dists, int64_t* out_counts, eps_stats* stats) {
   Index* ix = reinterpret_cast<Index*>(h);
   if (!ix || !queries || !out_ids || !out_dists || !out_counts) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null argument");
+  EPS_TRY(eps::dense_only(ix));
   if (nq <= 0) return EPS_OK;
   if (limit < 1) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "limit must be >= 1");
   EPS_TRY(eps::check_device(ix->device));
@@ -675,6 +755,73 @@ int eps_search_batch(eps_index* h, const float* queries, int64_t nq, int64_t lim
     stats->total_ms += ms;
   }
   ix->graph_counters_pending = false;
+  return EPS_OK;
+}
+
+int eps_index_append_sparse_rows(eps_index* h, int64_t first_row, int64_t n_rows, const int64_t* offsets,
+                                 const int64_t* indices, const float* values) {
+  Index* ix = reinterpret_cast<Index*>(h);
+  if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");
+  if (!ix->sparse) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "sparse rows appended to a dense index");
+  EPS_TRY(eps::check_device(ix->device));
+  EPS_TRY(check_mutable(ix));
+  return eps::sparse_append(ix, first_row, n_rows, offsets, indices, values);
+}
+
+int eps_search_sparse_batch(eps_index* h, int64_t nq, const int64_t* q_offsets, const int64_t* q_indices, const float* q_values,
+                            int64_t limit, const eps_filter_node* filter, int64_t n_filter, int64_t* out_ids, double* out_dists,
+                            int64_t* out_counts, eps_stats* stats) {
+  Index* ix = reinterpret_cast<Index*>(h);
+  if (!ix || !out_ids || !out_dists || !out_counts) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null argument");
+  if (!ix->sparse) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "sparse search on a dense index");
+  if (nq <= 0) return EPS_OK;
+  if (!q_offsets) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null query offsets");
+  if (limit < 1) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "limit must be >= 1");
+  EPS_TRY(eps::check_device(ix->device));
+  // queries: any index the 32-bit element holds (the merge needs them strictly increasing)
+  std::vector<int64_t> qp;
+  std::vector<uint2> qe;
+  std::vector<float> qn;
+  EPS_TRY(eps::pack_sparse(nq, q_offsets, q_indices, q_values, 0xffffffffll, 0, &qp, &qe, &qn));
+  if (stats) EPS_CUDA(cudaEventRecord(ix->ev[0], ix->stream));
+  // one device block [ptr | norm2 | elems] in, one block [ids | counts | dists] out through a pinned host mirror
+  const size_t ptr_bytes = static_cast<size_t>(nq + 1) * 8, nrm_off = ptr_bytes,
+               el_off = nrm_off + ((static_cast<size_t>(nq) * 4 + 7) & ~static_cast<size_t>(7));
+  EPS_TRY(ix->s_sparse_q.reserve(el_off + qe.size() * 8));
+  unsigned char* d_q = ix->s_sparse_q.as<unsigned char>();
+  EPS_CUDA(cudaMemcpyAsync(d_q, qp.data(), ptr_bytes, cudaMemcpyHostToDevice, ix->stream));
+  EPS_CUDA(cudaMemcpyAsync(d_q + nrm_off, qn.data(), static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, ix->stream));
+  if (!qe.empty()) EPS_CUDA(cudaMemcpyAsync(d_q + el_off, qe.data(), qe.size() * 8, cudaMemcpyHostToDevice, ix->stream));
+  const size_t n_ids = static_cast<size_t>(nq) * limit;
+  const size_t off_cnt = n_ids * 8, off_dist = off_cnt + static_cast<size_t>(nq) * 8, total = off_dist + n_ids * 4;
+  EPS_TRY(ix->s_out_ids.reserve(total));
+  if (ix->h_out_cap < total) {
+    if (ix->h_out) cudaFreeHost(ix->h_out);
+    ix->h_out = nullptr;
+    ix->h_out_cap = 0;
+    EPS_CUDA(cudaHostAlloc(&ix->h_out, total, cudaHostAllocDefault));
+    ix->h_out_cap = total;
+  }
+  unsigned char* d_blk = ix->s_out_ids.as<unsigned char>();
+  const eps::SparseQueries q{reinterpret_cast<const int64_t*>(d_q), reinterpret_cast<const uint2*>(d_q + el_off),
+                             reinterpret_cast<const float*>(d_q + nrm_off)};
+  EPS_TRY(eps::search_sparse_device(ix, q, nq, limit, filter, n_filter, reinterpret_cast<int64_t*>(d_blk),
+                                    reinterpret_cast<float*>(d_blk + off_dist), reinterpret_cast<int64_t*>(d_blk + off_cnt), stats));
+  EPS_CUDA(cudaMemcpyAsync(ix->h_out, d_blk, total, cudaMemcpyDeviceToHost, ix->stream));
+  if (stats) EPS_CUDA(cudaEventRecord(ix->ev[3], ix->stream));
+  EPS_CUDA(cudaStreamSynchronize(ix->stream));
+  const unsigned char* hb = static_cast<const unsigned char*>(ix->h_out);
+  std::memcpy(out_ids, hb, n_ids * 8);
+  std::memcpy(out_counts, hb + off_cnt, static_cast<size_t>(nq) * 8);
+  const float* hd = reinterpret_cast<const float*>(hb + off_dist);
+  for (size_t i = 0; i < n_ids; ++i) out_dists[i] = static_cast<double>(hd[i]);
+  if (stats) {
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, ix->ev[1], ix->ev[2]);
+    stats->kernel_ms += ms;
+    cudaEventElapsedTime(&ms, ix->ev[0], ix->ev[3]);
+    stats->total_ms += ms;
+  }
   return EPS_OK;
 }
 
@@ -727,6 +874,7 @@ int eps_pair_distances(int device, int metric, const float* a, const float* b, i
 int eps_index_set_search_width(eps_index* h, int width) {
   Index* ix = reinterpret_cast<Index*>(h);
   if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");
+  EPS_TRY(eps::dense_only(ix));
   if (width < 1 || width > 8) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "search width must be in [1, 8]");
   ix->search_width = width;
   return EPS_OK;
@@ -735,6 +883,7 @@ int eps_index_set_search_width(eps_index* h, int width) {
 int eps_index_set_graph_tuning(eps_index* h, int ring_slots, int ctas_per_sm) {
   Index* ix = reinterpret_cast<Index*>(h);
   if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");
+  EPS_TRY(eps::dense_only(ix));
   if (ring_slots < 0 || ring_slots > 24 || ctas_per_sm < 0 || ctas_per_sm > 32)
     return eps::fail(EPS_ERR_INVALID_ARGUMENT, "ring_slots must be in [0, 24] and ctas_per_sm in [0, 32] (0 = auto)");
   ix->graph_ring_slots = ring_slots;
@@ -745,6 +894,7 @@ int eps_index_set_graph_tuning(eps_index* h, int ring_slots, int ctas_per_sm) {
 int eps_index_set_coarse(eps_index* h, int mode) {
   Index* ix = reinterpret_cast<Index*>(h);
   if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");
+  EPS_TRY(eps::dense_only(ix));
   if (mode < 0 || mode > 2) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "coarse mode must be 0 (fp32), 1 (tf32) or 2 (bf16)");
   if (mode != ix->coarse_mode) ix->coarse_boost = 1;  // the learnt k' multiplier belongs to one operand format
   ix->coarse_mode = mode;
@@ -758,7 +908,11 @@ int eps_index_set_coarse_guard(eps_index* h, int on) {
   return EPS_OK;
 }
 
-const float* eps_index_device_rows(eps_index* h) { return h ? reinterpret_cast<Index*>(h)->d_vectors : nullptr; }
+const float* eps_index_device_rows(eps_index* h) {
+  if (!h) return nullptr;
+  if (eps::dense_only(reinterpret_cast<Index*>(h)) != EPS_OK) return nullptr;
+  return reinterpret_cast<Index*>(h)->d_vectors;
+}
 int64_t eps_index_rows(eps_index* h) { return h ? reinterpret_cast<Index*>(h)->n_rows : 0; }
 
 void* eps_index_stream(eps_index* h) { return h ? reinterpret_cast<Index*>(h)->stream : nullptr; }

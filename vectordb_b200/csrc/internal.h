@@ -45,6 +45,13 @@ struct Index {
   int64_t n_rows = 0;           // rows mirrored so far (record_number_ snapshot)
   bool vec4 = false;            // dim % 4 == 0 and 16-B aligned base
 
+  // sparse column (eps_index_create_sparse): rows are a CSR of {uint32 index, float value} elements
+  bool sparse = false;
+  int64_t* d_sp_ptr = nullptr;  // [sp_row_cap + 1] element offsets of the rows
+  uint2* d_sp_elems = nullptr;  // [sp_elem_cap] {index, value bits}, indices strictly increasing within a row
+  float* d_sp_norm2 = nullptr;  // [sp_row_cap] sequential fp32 sum of squares of each row (cosine)
+  int64_t sp_nnz = 0, sp_elem_cap = 0, sp_row_cap = 0;
+
   // graph (ANNGraphSegment mirror)
   int64_t n_indexed = 0;
   int64_t n_edges = 0;
@@ -83,7 +90,8 @@ struct Index {
 
   // scratch
   DevBuf s_queries, s_dist, s_topk, s_topk2, s_pass, s_filter, s_vset, s_visited, s_vlog, s_queue, s_tail, s_out_ids, s_out_dists,
-      s_out_counts, s_stats, s_misc, s_seed_rows, s_seed_dist, s_xnorm, s_qnorm, s_coarse, s_thr, s_cand, s_cand_cnt, s_bf16, s_qbf16, s_flags;
+      s_out_counts, s_stats, s_misc, s_seed_rows, s_seed_dist, s_xnorm, s_qnorm, s_coarse, s_thr, s_cand, s_cand_cnt, s_bf16, s_qbf16, s_flags,
+      s_sparse_q;
   int coarse_mode = 1;           // exact-scan coarse pass: 0 = fp32 SIMT only, 1 = wgmma TF32, 2 = wgmma bf16 mirror
   int coarse_guard = 1;          // verify the coarse pass after the re-score and redo unsafe queries (brute_force.cu)
   int coarse_boost = 1;          // multiplier of k' learnt by the guard for this table (1, 4, 16, 64)
@@ -133,6 +141,40 @@ int tc_launch_distances(Index* ix, int64_t row_start, int64_t n, const float* d_
 int brute_force_knn_rows(Index* ix, int64_t q_start, int64_t nq, int64_t n_rows, int64_t k,
                          unsigned long long* d_topk, eps_stats* stats);
 
+// Producer of the [nq x ldd] fp32 distance tile of rows [row_start, row_start + n) that the exact scan selects from,
+// in place of launch_distances (the sparse scan, sparse.cu).
+struct DistProducer {
+  virtual ~DistProducer() = default;
+  virtual int launch(Index* ix, int64_t row_start, int64_t n, float* D, int64_t ldd, uint64_t* launches) const = 0;
+};
+// brute_force_topk with the distances of `dist` (nq queries): same pass bitmap, selection and key layout, never the
+// tensor-core pass.  self_base >= 0 excludes row self_base + q from query q's list (the build's kNN lists).
+int scan_topk(Index* ix, const DistProducer& dist, int64_t nq, int64_t row_start, int64_t row_end, int64_t k,
+              const FilterProg* d_prog, const FilterProg* h_prog, bool prefilter, int64_t self_base,
+              unsigned long long* d_topk, eps_stats* stats);
+
+// ---- sparse.cu -----------------------------------------------------------------------------
+// Queries of the sparse scan as a device CSR: ptr[q] .. ptr[q+1] index elems (absolute offsets), norm2[q] = the
+// sequential fp32 sum of squares.
+struct SparseQueries {
+  const int64_t* ptr;
+  const uint2* elems;
+  const float* norm2;
+};
+struct SparseDist : DistProducer {
+  SparseQueries q;
+  int64_t nq;
+  int metric;
+  int launch(Index* ix, int64_t row_start, int64_t n, float* D, int64_t ldd, uint64_t* launches) const override;
+};
+// Validate and pack n rows of a caller CSR (offsets[0..n], indices, values) into ptr (n+1 entries, starting at
+// ptr_base), elems and norm2.  Indices must be >= 0, < max_index and strictly increasing within a row.
+int pack_sparse(int64_t n, const int64_t* offsets, const int64_t* indices, const float* values, int64_t max_index,
+                int64_t ptr_base, std::vector<int64_t>* ptr, std::vector<uint2>* elems, std::vector<float>* norm2);
+int sparse_append(Index* ix, int64_t first_row, int64_t n_rows, const int64_t* offsets, const int64_t* indices,
+                  const float* values);
+int build_graph_sparse(Index* ix, int64_t n, const eps_build_params* params);
+
 // ---- graph_search.cu -----------------------------------------------------------------------
 // Best-first search of nq queries over the installed CSR graph with queue length L (<= n_indexed).
 // Output: d_queue [nq x L] sorted keys.
@@ -160,6 +202,30 @@ int merge_shards(int device, cudaStream_t stream, const int64_t* d_ids, const fl
 
 // ---- build.cu ------------------------------------------------------------------------------
 int build_graph(Index* ix, int64_t n, const eps_build_params* params);
+// Install a host CSR (int64 offsets, int32 ids) as the index's graph, dropping everything derived from the old one.
+int install_csr(Index* ix, int64_t n, const int64_t* off, const int32_t* nb, int64_t e, int64_t nav);
+
+// Connectivity repair of a build (CheckConnectivity, nsg.cpp:687-775) on host lists: the integer-only steps.
+// lists: [n x stride] out-neighbours, cnt[v] of them valid; knn: [n x K] sorted keys (kKeyInf padded).
+struct ConnRepair {
+  int64_t n;
+  const int32_t* lists;
+  const int32_t* cnt;
+  int stride;
+  std::vector<uint8_t> seen;
+  std::vector<int32_t> stack;
+  int64_t linked = 0;
+  std::vector<std::vector<int32_t>> extra;  // edges added by the repair
+  std::vector<int32_t> entries;             // one per component that the kNN lists do not connect to the rest
+  ConnRepair(int64_t n_, const int32_t* lists_, const int32_t* cnt_, int stride_);
+  void flood(int32_t root);
+  // steps 1 and 2: attach every unlinked vertex to its nearest linked kNN entry with room, or make it an entry
+  void attach_from_knn(const unsigned long long* knn, int K);
+  // step 4: attach u to a random linked vertex (rng: the build's LCG state)
+  void attach_random(int32_t u, uint64_t* rng);
+  // entries become out-neighbours of nav; flatten lists + extra edges to the reference CSR
+  void flatten(int64_t nav, std::vector<int64_t>* off, std::vector<int32_t>* nb);
+};
 
 // ---- misc kernels (capi.cu) ----------------------------------------------------------------
 int normalize_rows_device(cudaStream_t s, float* d, int64_t n, int64_t dim);

@@ -139,6 +139,7 @@ int eps_search_batch_sharded(eps_shard_group* gh, eps_index* h, int64_t id_base,
   ShardGroup* g = reinterpret_cast<ShardGroup*>(gh);
   Index* ix = reinterpret_cast<Index*>(h);
   if (!g || !ix || !d_queries || !d_out_ids || !d_out_dists) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null argument");
+  if (ix->sparse) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "sharded search of a sparse index is not supported");
   if (nq <= 0) return EPS_OK;
   if (k < 1) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "k must be >= 1");
   if (ix->device != g->device) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "index and shard group live on different devices");

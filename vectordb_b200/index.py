@@ -189,6 +189,68 @@ class Index:
         return self.L.eps_index_stream(self.h)
 
 
+def as_csr(rows):
+    """scipy CSR matrix or (offsets, indices, values) -> contiguous (int64 offsets, int64 indices, float32 values)."""
+    if hasattr(rows, "indptr") and hasattr(rows, "indices") and hasattr(rows, "data"):
+        m = rows.tocsr()
+        if not m.has_sorted_indices:
+            m = m.sorted_indices()
+        offsets, indices, values = m.indptr, m.indices, m.data
+    else:
+        offsets, indices, values = rows
+    return (np.ascontiguousarray(offsets, np.int64), np.ascontiguousarray(indices, np.int64),
+            np.ascontiguousarray(values, np.float32))
+
+
+class SparseIndex(Index):
+    """Device mirror of one sparse-vector field (eps_index_create_sparse): rows are appended as CSR, searches are
+    exact scans.  Config, deleted bits, attributes, string codes, facets, build and get_graph work as on Index."""
+
+    def __init__(self, metric, dim, capacity=0, device=0):
+        self.L = load_library()
+        self.metric = METRICS[metric] if isinstance(metric, str) else int(metric)
+        self.dim = int(dim)
+        self.device = device
+        self._host = None
+        self.capacity = int(capacity or 0)
+        self._keep = []
+        h = C.c_void_p()
+        check(self.L.eps_index_create_sparse(C.byref(h), self.metric, self.dim, self.capacity, device))
+        self.h = h
+
+    def view(self):
+        v = SparseIndex.__new__(SparseIndex)
+        v.L, v.metric, v.dim, v.device, v._host, v.capacity, v._keep = self.L, self.metric, self.dim, self.device, None, self.capacity, []
+        h = C.c_void_p()
+        check(self.L.eps_index_create_view(self.h, C.byref(h)))
+        v.h = h
+        v._base = self
+        return v
+
+    @property
+    def rows(self):
+        return int(self.L.eps_index_rows(self.h))
+
+    def append(self, rows, first_row=None):
+        """Append CSR rows (scipy CSR or (offsets, indices, values)) after the rows already mirrored."""
+        off, idx, val = as_csr(rows)
+        first = self.rows if first_row is None else int(first_row)
+        check(self.L.eps_index_append_sparse_rows(self.h, first, off.size - 1, _p(off), _p(idx), _p(val)))
+
+    def search(self, queries, limit, filter_nodes=None, want_stats=True):
+        """Exact scan of CSR queries (eps_search_sparse_batch).  Returns ids [nq,limit], dists float64, counts, Stats."""
+        off, idx, val = as_csr(queries)
+        nq = off.size - 1
+        ids = np.empty((nq, limit), np.int64)
+        dists = np.empty((nq, limit), np.float64)
+        counts = np.empty(nq, np.int64)
+        st = StatsStruct()
+        arr, n = filter_nodes_array(filter_nodes)
+        check(self.L.eps_search_sparse_batch(self.h, nq, _p(off), _p(idx), _p(val), int(limit), arr, n, _p(ids), _p(dists),
+                                             _p(counts), C.byref(st) if want_stats else None))
+        return ids, dists, counts, Stats.from_struct(st)
+
+
 def normalize(vectors, device=0):
     v = np.ascontiguousarray(vectors, np.float32).copy()
     if v.ndim == 1:

@@ -290,17 +290,31 @@ EPS_API int eps_index_append_sparse_rows(eps_index* ix, int64_t first_row, int64
  * output contract of eps_search_batch.  Distances are bit-identical to GetL2DistSqr / GetInnerProductDist /
  * GetCosineDist (db/vector.cpp:7-100, row = v1, query = v2): the same sequential fp32 sums in the same order, no FMA.
  * Cosine queries must already be normalised (db/table_mvp.cpp:337-349), like dense ones.
- * A sparse index ALWAYS answers by the exact scan over all mirrored rows, with the reference's brute-force caps
- * (prefilter / force_brute: limit results; otherwise min(limit, L_local)), even when a graph is installed.  This is
- * the one deliberate deviation from the reference: where it would search its graph (n_indexed >= 512), the GPU returns
- * the exact top-k.  Cosine with an empty row or an empty query gives 0/0 = NaN (the reference's std::sort order of
- * such entries is unspecified): NaN distances sort after every number.  eps_stats.n_dist counts nq x the rows scanned.
+ * In the default mode (EPS_SPARSE_SEARCH_SCAN) a sparse index ALWAYS answers by the exact scan over all mirrored rows,
+ * with the reference's brute-force caps (prefilter / force_brute: limit results; otherwise min(limit, L_local)), even
+ * when a graph is installed.  This is the one deliberate deviation from the reference: where it would search its graph
+ * (n_indexed >= 512), the GPU returns the exact top-k.  eps_stats.n_dist counts nq x the rows scanned.
+ * In EPS_SPARSE_SEARCH_GRAPH mode (eps_index_set_sparse_search) the index follows the reference's branch rule: prefilter,
+ * force_brute or n_indexed < 512 select the same exact scan; otherwise the installed graph over rows [0, n_indexed) is
+ * searched with queue length min(L_master, n_indexed) in the reference's sequential order (IntraQueryThreads = 1), rows
+ * [n_indexed, total) are scanned, and the two are merged and post-filtered as Search does (:885-927).  The ids, the
+ * distances (bitwise) and the distance-evaluation counts are then those of the reference at IntraQueryThreads = 1;
+ * eps_stats.n_dist counts seeds, fresh neighbours and tail rows, n_seed the seeds, n_expand / n_edges the expansions
+ * and the adjacency entries they read.
+ * Cosine with an empty row or an empty query gives 0/0 = NaN (the reference's std::sort order of such entries is
+ * unspecified): NaN distances sort after every number.
  * eps_index_build on a sparse index installs the exact out_degree-NN lists (field metric, self excluded), the L2
  * nearest row to the reference's sparse centre (nsg.cpp:120-135) as navigation point, and repair edges that make every
  * row reachable from it.  HOST buffers in and out. */
 EPS_API int eps_search_sparse_batch(eps_index* ix, int64_t nq, const int64_t* q_offsets, const int64_t* q_indices,
                                     const float* q_values, int64_t limit, const eps_filter_node* filter, int64_t n_filter,
                                     int64_t* out_ids, double* out_dists, int64_t* out_counts, eps_stats* stats);
+
+/* How eps_search_sparse_batch answers on a sparse index (see there).  A view starts with its base's mode and may set
+ * its own.  A dense index or an unknown mode: EPS_ERR_INVALID_ARGUMENT. */
+#define EPS_SPARSE_SEARCH_SCAN 0   /* default: the exact scan always */
+#define EPS_SPARSE_SEARCH_GRAPH 1  /* the reference's branch rule: graph search + tail scan where it searches its graph */
+EPS_API int eps_index_set_sparse_search(eps_index* ix, int mode);
 
 /* Raw stream handle (cudaStream_t) the index launches on, for callers that time with CUDA events. */
 EPS_API void* eps_index_stream(eps_index* ix);

@@ -179,6 +179,71 @@ int bind_program_columns(Index* ix, FilterProg* prog) {
   return EPS_OK;
 }
 
+// What the graph branch of Search needs from a query batch: the graph search of its queries over [0, n_indexed), and
+// the exact top-k of rows [n_indexed, total) that feeds the tail merge.
+struct GraphQueries {
+  virtual ~GraphQueries() = default;
+  virtual int search(Index* ix, int64_t L, unsigned long long* d_queue, eps_stats* st) const = 0;
+  virtual int tail(Index* ix, int64_t k, const FilterProg* d_prog, const FilterProg* h_prog, unsigned long long* d_tail,
+                   eps_stats* st) const = 0;
+};
+
+struct DenseGraphQueries : GraphQueries {
+  const float* d_queries;
+  int64_t nq;
+  DenseGraphQueries(const float* q, int64_t n) : d_queries(q), nq(n) {}
+  int search(Index* ix, int64_t L, unsigned long long* d_queue, eps_stats* st) const override {
+    return graph_search(ix, d_queries, nq, L, d_queue, st);
+  }
+  int tail(Index* ix, int64_t k, const FilterProg* d_prog, const FilterProg* h_prog, unsigned long long* d_tail,
+           eps_stats* st) const override {
+    return brute_force_topk(ix, d_queries, nq, ix->n_indexed, ix->n_rows, k, d_prog, h_prog, false, d_tail, st);
+  }
+};
+
+struct SparseGraphQueries : GraphQueries {
+  SparseDist dist;
+  explicit SparseGraphQueries(const SparseDist& d) : dist(d) {}
+  int search(Index* ix, int64_t L, unsigned long long* d_queue, eps_stats* st) const override {
+    return sparse_graph_search(ix, dist.q, dist.nq, L, d_queue, st);
+  }
+  int tail(Index* ix, int64_t k, const FilterProg* d_prog, const FilterProg* h_prog, unsigned long long* d_tail,
+           eps_stats* st) const override {
+    return scan_topk(ix, dist, dist.nq, ix->n_indexed, ix->n_rows, k, d_prog, h_prog, false, -1, d_tail, st);
+  }
+};
+
+// The graph branch of Search (:869-933): graph search, exact scan of the rows appended after the build, merge of the
+// two and post-filter walk.  ev[2] is recorded after the graph search when stats are wanted.
+static int graph_branch(Index* ix, const GraphQueries& gq, int64_t nq, int64_t limit, const FilterProg* d_prog,
+                        const FilterProg* h_prog, int64_t* d_ids, float* d_dists, int64_t* d_counts, eps_stats* stats,
+                        eps_stats* local) {
+  const int64_t total = ix->n_rows;
+  const int64_t n_indexed = ix->n_indexed;
+  const int64_t L = std::min<int64_t>(ix->L_master, n_indexed);  // Q1 clamp
+  // :872 min(n_indexed, limit, L_local); the queue row holds L entries, so the merge window is clamped to it
+  // (the reference ties L_local to L_master through setSearchQueueSize; the C ABI accepts them separately)
+  const int64_t search_limit = std::min<int64_t>(std::min<int64_t>(std::min<int64_t>(n_indexed, limit), ix->L_local), L);
+  EPS_TRY(ix->s_queue.reserve(static_cast<size_t>(nq) * L * 8));
+  EPS_TRY(gq.search(ix, L, ix->s_queue.as<unsigned long long>(), local));
+  ix->graph_counters_pending = true;
+  if (stats) EPS_CUDA(cudaEventRecord(ix->ev[2], ix->stream));
+  const unsigned long long* d_tail = nullptr;
+  int64_t tail_k = 0;
+  if (total > n_indexed) {  // :885-900
+    // only the first search_limit slots can receive tail entries (:894-900)
+    tail_k = std::min<int64_t>(std::min<int64_t>(limit, total - n_indexed), search_limit);
+    if (tail_k > 8192) return fail(EPS_ERR_UNSUPPORTED, "more than 8192 tail results per query are not supported");
+    EPS_TRY(ix->s_tail.reserve(static_cast<size_t>(nq) * tail_k * 8));
+    EPS_TRY(gq.tail(ix, tail_k, d_prog, h_prog, ix->s_tail.as<unsigned long long>(), local));
+    d_tail = ix->s_tail.as<unsigned long long>();
+  }
+  EPS_TRY(finalize_graph(ix, ix->s_queue.as<unsigned long long>(), nq, L, search_limit, L, d_tail, tail_k, limit,
+                         d_prog, h_prog, d_ids, d_dists, d_counts));
+  local->kernel_launches += 1;
+  return EPS_OK;
+}
+
 static int search_device(Index* ix, const float* d_queries, int64_t nq, int64_t limit, const eps_filter_node* filter,
                          int64_t n_filter, int64_t* d_ids, float* d_dists, int64_t* d_counts, eps_stats* stats) {
   if (nq <= 0) return EPS_OK;
@@ -213,28 +278,8 @@ static int search_device(Index* ix, const float* d_queries, int64_t nq, int64_t 
     EPS_TRY(finalize_keys(ix, ix->s_topk.as<unsigned long long>(), nq, k, limit, cap, d_ids, d_dists, d_counts));
     local.kernel_launches += 1;
   } else {
-    const int64_t L = std::min<int64_t>(ix->L_master, n_indexed);  // Q1 clamp
-    // :872 min(n_indexed, limit, L_local); the queue row holds L entries, so the merge window is clamped to it
-    // (the reference ties L_local to L_master through setSearchQueueSize; the C ABI accepts them separately)
-    const int64_t search_limit = std::min<int64_t>(std::min<int64_t>(std::min<int64_t>(n_indexed, limit), ix->L_local), L);
-    EPS_TRY(ix->s_queue.reserve(static_cast<size_t>(nq) * L * 8));
-    EPS_TRY(graph_search(ix, d_queries, nq, L, ix->s_queue.as<unsigned long long>(), &local));
-    ix->graph_counters_pending = true;
-    if (stats) EPS_CUDA(cudaEventRecord(ix->ev[2], ix->stream));
-    const unsigned long long* d_tail = nullptr;
-    int64_t tail_k = 0;
-    if (total > n_indexed) {  // :885-900
-      // only the first search_limit slots can receive tail entries (:894-900)
-      tail_k = std::min<int64_t>(std::min<int64_t>(limit, total - n_indexed), search_limit);
-      if (tail_k > 8192) return fail(EPS_ERR_UNSUPPORTED, "more than 8192 tail results per query are not supported");
-      EPS_TRY(ix->s_tail.reserve(static_cast<size_t>(nq) * tail_k * 8));
-      EPS_TRY(brute_force_topk(ix, d_queries, nq, n_indexed, total, tail_k, d_prog, &h_prog, false,
-                               ix->s_tail.as<unsigned long long>(), &local));
-      d_tail = ix->s_tail.as<unsigned long long>();
-    }
-    EPS_TRY(finalize_graph(ix, ix->s_queue.as<unsigned long long>(), nq, L, search_limit, L, d_tail, tail_k, limit,
-                           d_prog, &h_prog, d_ids, d_dists, d_counts));
-    local.kernel_launches += 1;
+    EPS_TRY(graph_branch(ix, DenseGraphQueries(d_queries, nq), nq, limit, d_prog, &h_prog, d_ids, d_dists, d_counts, stats,
+                         &local));
   }
   if (stats) {
     stats->n_dist += local.n_dist;
@@ -248,8 +293,9 @@ static int search_device(Index* ix, const float* d_queries, int64_t nq, int64_t 
   return EPS_OK;
 }
 
-// search_device for a sparse index: always the exact scan over [0, total) with the brute-force branch's caps
-// (:857 prefilter: limit; :864 brute: min(limit, L_local)), whatever graph is installed.
+// search_device for a sparse index.  EPS_SPARSE_SEARCH_SCAN: always the exact scan over [0, total) with the brute-force
+// branch's caps (:857 prefilter: limit; :864 brute: min(limit, L_local)), whatever graph is installed.
+// EPS_SPARSE_SEARCH_GRAPH: the reference's branch rule (:855-868), the graph branch where it applies.
 static int search_sparse_device(Index* ix, const SparseQueries& q, int64_t nq, int64_t limit, const eps_filter_node* filter,
                                 int64_t n_filter, int64_t* d_ids, float* d_dists, int64_t* d_counts, eps_stats* stats) {
   if (nq <= 0) return EPS_OK;
@@ -263,23 +309,32 @@ static int search_sparse_device(Index* ix, const SparseQueries& q, int64_t nq, i
     d_prog = ix->s_filter.as<FilterProg>();
   }
   const int64_t total = ix->n_rows;
-  const int64_t cap = (ix->prefilter || ix->force_brute) ? limit : std::min<int64_t>(limit, ix->L_local);
-  const int64_t k = std::max<int64_t>(1, std::min<int64_t>(cap, total));
-  if (k > 8192) return fail(EPS_ERR_UNSUPPORTED, "more than 8192 results per query from the exact scan are not supported");
-  eps_stats local;
-  std::memset(&local, 0, sizeof(local));
-  if (stats) EPS_CUDA(cudaEventRecord(ix->ev[1], ix->stream));
-  EPS_TRY(ix->s_topk.reserve(static_cast<size_t>(nq) * k * 8));
   SparseDist dist;
   dist.q = q;
   dist.nq = nq;
   dist.metric = ix->metric;
-  EPS_TRY(scan_topk(ix, dist, nq, 0, total, k, d_prog, &h_prog, ix->prefilter, -1, ix->s_topk.as<unsigned long long>(), &local));
-  if (stats) EPS_CUDA(cudaEventRecord(ix->ev[2], ix->stream));
-  EPS_TRY(finalize_keys(ix, ix->s_topk.as<unsigned long long>(), nq, k, limit, cap, d_ids, d_dists, d_counts));
-  local.kernel_launches += 1;
+  eps_stats local;
+  std::memset(&local, 0, sizeof(local));
+  if (stats) EPS_CUDA(cudaEventRecord(ix->ev[1], ix->stream));
+  const bool graph = ix->sparse_search == EPS_SPARSE_SEARCH_GRAPH && !ix->prefilter && !ix->force_brute &&
+                     ix->n_indexed >= 512;  // BruteforceThreshold (hpp:28)
+  if (graph) {
+    EPS_TRY(graph_branch(ix, SparseGraphQueries(dist), nq, limit, d_prog, &h_prog, d_ids, d_dists, d_counts, stats, &local));
+  } else {
+    const int64_t cap = (ix->prefilter || ix->force_brute) ? limit : std::min<int64_t>(limit, ix->L_local);
+    const int64_t k = std::max<int64_t>(1, std::min<int64_t>(cap, total));
+    if (k > 8192) return fail(EPS_ERR_UNSUPPORTED, "more than 8192 results per query from the exact scan are not supported");
+    EPS_TRY(ix->s_topk.reserve(static_cast<size_t>(nq) * k * 8));
+    EPS_TRY(scan_topk(ix, dist, nq, 0, total, k, d_prog, &h_prog, ix->prefilter, -1, ix->s_topk.as<unsigned long long>(), &local));
+    if (stats) EPS_CUDA(cudaEventRecord(ix->ev[2], ix->stream));
+    EPS_TRY(finalize_keys(ix, ix->s_topk.as<unsigned long long>(), nq, k, limit, cap, d_ids, d_dists, d_counts));
+    local.kernel_launches += 1;
+  }
   if (stats) {
     stats->n_dist += local.n_dist;
+    stats->n_seed += local.n_seed;
+    stats->n_expand += local.n_expand;
+    stats->n_edges += local.n_edges;
     stats->n_queries += static_cast<uint64_t>(nq);
     stats->kernel_launches += local.kernel_launches;
   }
@@ -433,7 +488,7 @@ int eps_index_create_view(eps_index* base_h, eps_index** out) {
   ix->attr_cap_rows = base->attr_cap_rows;
   for (int i = 0; i < eps::kMaxStringCols; ++i) ix->str_cols[i] = base->str_cols[i];
   ix->L_master = base->L_master; ix->L_local = base->L_local; ix->prefilter = base->prefilter; ix->force_brute = base->force_brute;
-  ix->search_width = base->search_width; ix->graph_ring_slots = base->graph_ring_slots;
+  ix->search_width = base->search_width; ix->sparse_search = base->sparse_search; ix->graph_ring_slots = base->graph_ring_slots;
   ix->graph_ctas_per_sm = base->graph_ctas_per_sm; ix->num_sms = base->num_sms;
   ix->coarse_mode = base->coarse_mode; ix->coarse_guard = base->coarse_guard; ix->coarse_boost = base->coarse_boost;
   cudaError_t e = cudaStreamCreateWithFlags(&ix->stream, cudaStreamNonBlocking);
@@ -816,12 +871,14 @@ int eps_search_sparse_batch(eps_index* h, int64_t nq, const int64_t* q_offsets, 
   const float* hd = reinterpret_cast<const float*>(hb + off_dist);
   for (size_t i = 0; i < n_ids; ++i) out_dists[i] = static_cast<double>(hd[i]);
   if (stats) {
+    if (ix->graph_counters_pending) EPS_TRY(eps::read_graph_counters(ix, stats));
     float ms = 0.f;
     cudaEventElapsedTime(&ms, ix->ev[1], ix->ev[2]);
     stats->kernel_ms += ms;
     cudaEventElapsedTime(&ms, ix->ev[0], ix->ev[3]);
     stats->total_ms += ms;
   }
+  ix->graph_counters_pending = false;
   return EPS_OK;
 }
 
@@ -877,6 +934,16 @@ int eps_index_set_search_width(eps_index* h, int width) {
   EPS_TRY(eps::dense_only(ix));
   if (width < 1 || width > 8) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "search width must be in [1, 8]");
   ix->search_width = width;
+  return EPS_OK;
+}
+
+int eps_index_set_sparse_search(eps_index* h, int mode) {
+  Index* ix = reinterpret_cast<Index*>(h);
+  if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");
+  if (!ix->sparse) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "sparse search mode on a dense index");
+  if (mode != EPS_SPARSE_SEARCH_SCAN && mode != EPS_SPARSE_SEARCH_GRAPH)
+    return eps::fail(EPS_ERR_INVALID_ARGUMENT, "sparse search mode must be 0 (scan) or 1 (graph)");
+  ix->sparse_search = mode;
   return EPS_OK;
 }
 

@@ -44,14 +44,13 @@
 #include <cstdlib>
 
 #include "async.cuh"
+#include "graph_search.cuh"
 #include "internal.h"
 
 namespace eps {
 
 constexpr int kEll = 64;        // adjacency ids per fixed-stride row
-constexpr int kGsThreads = 128;
 constexpr int kMaxW = 8;        // candidates picked per iteration (upper bound)
-constexpr int kPC = 128;        // accepted keys pending their merge (= one key per thread in the merge)
 constexpr int kMaxS = 8;        // ring slots per consumer warp (upper bound)
 constexpr int kMaxR = 24;       // ring slots (upper bound: 3 consumer warps x kMaxS)
 constexpr int kRounds = kMaxW * kEll / kGsThreads;  // adjacency slots per thread
@@ -96,36 +95,6 @@ struct GSArgs {
   unsigned long long* qtimes;     // developer build: [nq x 2] globaltimer at query start / end (null otherwise)
   int slot_bytes;                 // ring slot pitch (row bytes, multiple of 16); 0 when rows are not staged
 };
-
-__device__ __forceinline__ int lb_masked(const unsigned long long* a, int n, unsigned long long key) {
-  int lo = 0, hi = n;
-  while (lo < hi) {
-    int mid = (lo + hi) >> 1;
-    if ((a[mid] & kKeyMask) < key) lo = mid + 1; else hi = mid;
-  }
-  return lo;
-}
-
-// Visited hash set: linear probing over the entries of a slot's table from the first entry of the id's bucket
-// (multiplicative hash).  Entries go from kVsetEmpty to an id once and stay until the table is refilled after the
-// query, so an id found anywhere is visited, and an entry seen holding another id stays so.  Reads bypass L1
-// (__ldcg): the entries are written by L2 atomics.
-constexpr uint32_t kVsetEmpty = 0xffffffffu;  // ids are < 2^31
-constexpr uint32_t kVsetMul = 0x9e3779b1u;
-__device__ __forceinline__ uint32_t vset_bucket(uint32_t id, int shift) { return ((id * kVsetMul) >> shift) << 3; }
-// Test-and-insert from entry p on, one atomicCAS per entry: true when the id was absent (this thread inserted it).
-// Terminates because a query never fills its table beyond 3/4.  `acc` counts table accesses (developer build).
-__device__ __forceinline__ bool vset_claim(uint32_t* t, uint32_t mask, uint32_t p, uint32_t id, unsigned long long& acc) {
-  for (;;) {
-    const uint32_t old = atomicCAS(t + p, kVsetEmpty, id);
-#ifdef EPS_GS_PROFILE
-    ++acc;
-#endif
-    if (old == kVsetEmpty) return true;
-    if (old == id) return false;
-    p = (p + 1) & mask;
-  }
-}
 
 template <bool L2>
 __device__ __forceinline__ void acc4(const float4& x, const float4& y, float& a) {
@@ -242,64 +211,6 @@ __device__ __forceinline__ void consume_slots(const GSArgs& a, unsigned occ_mask
   if (lane < S && ((occ_mask >> lane) & 1u)) {
     const unsigned long long key = make_key(finish_metric(a.metric, mine), static_cast<uint32_t>(slot_id[cw + 3 * lane]));
     if (key < bound) pend[atomicAdd(s_npend, 1)] = key;  // dist > bound rejected (:424); ties by id
-  }
-}
-
-// Block-wide merge of the m (<= kPC) pending keys into the sorted queue qa[0..L): sort by counting, binary-search
-// the insertion points, shift the tail in place in super-tiles of 8 keys per thread (each key moves right by the
-// number of pending keys that precede it), drop the keys into the holes.  Entries pushed past L are evicted
-// (AddIntoQueue's drop-worst, :104-108).  Returns the lowest insert position through *s_cursor (min).
-__device__ __forceinline__ void merge_pending(unsigned long long* qa, unsigned long long* pend, unsigned long long* cs, int* pos,
-                                              int m, int L, int* s_npend, int* s_cursor, unsigned* ubits) {
-  const int tid = threadIdx.x;
-  if (tid < m) {
-    const unsigned long long key = pend[tid];
-    int r = 0;
-    for (int j = 0; j < m; ++j) r += ((pend[j] & kKeyMask) < (key & kKeyMask));
-    cs[r] = key;
-  }
-  __syncthreads();
-  if (tid < m) pos[tid] = lb_masked(qa, L, cs[tid] & kKeyMask);
-  __syncthreads();
-  const int p0 = pos[0];
-  for (int hi = L; hi > p0; hi -= 8 * kGsThreads) {
-    unsigned long long kreg[8];
-    int dreg[8];
-#pragma unroll
-    for (int u = 0; u < 8; ++u) {
-      const int j = hi - 1 - (u * kGsThreads + tid);
-      dreg[u] = L;
-      if (j >= p0) {
-        kreg[u] = qa[j];
-        int sft = 0;
-        if (m <= 8) { for (int i = 0; i < m; ++i) sft += (pos[i] <= j); }
-        else { int lo = 0, up = m; while (lo < up) { const int mid = (lo + up) >> 1; if (pos[mid] <= j) lo = mid + 1; else up = mid; } sft = lo; }
-        dreg[u] = j + sft;
-      }
-    }
-    __syncthreads();
-#pragma unroll
-    for (int u = 0; u < 8; ++u) if (dreg[u] < L) qa[dreg[u]] = kreg[u];
-    __syncthreads();
-  }
-  if (tid < m) {
-    const int f = pos[tid] + tid;
-    if (f < L) qa[f] = cs[tid];
-  }
-  if (tid == 0) {
-    *s_npend = 0;
-    if (p0 < *s_cursor) *s_cursor = p0;
-  }
-  __syncthreads();
-  // the unchecked-entry bitmap (one bit per queue slot, what the pick scans) from the first changed word on
-  if (p0 < L) {
-    const int nwords = (L + 31) >> 5, lane = tid & 31;
-    for (int w = (p0 >> 5) + (tid >> 5); w < nwords; w += kGsThreads / 32) {
-      const int idx = w * 32 + lane;
-      const unsigned b = __ballot_sync(kFull, idx < L && !(qa[idx] & kCheckedBit));
-      if (lane == 0) ubits[w] = b;
-    }
-    __syncthreads();
   }
 }
 
@@ -878,6 +789,57 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   int slots = static_cast<int>(std::min<int64_t>((nq + rounds - 1) / rounds, static_cast<int64_t>(per_sm) * ix->num_sms));
   if (ix->graph_ring_slots > 0 || ix->graph_ctas_per_sm > 0)  // tuning override: every resident slot, queries claimed dynamically
     slots = static_cast<int>(std::min<int64_t>(nq, static_cast<int64_t>(per_sm) * ix->num_sms));
+  VisitedSets vis;
+  EPS_TRY(prepare_visited(ix, slots, L, &vis));
+  EPS_TRY(ix->s_misc.reserve(256));  // [0..3] counters, [+32 B] work counter, [5] [30..31] developer hash-set counts,
+                                     // [8..24] developer phase timers, [25..29] developer prefix counts
+  EPS_CUDA(cudaMemsetAsync(ix->s_misc.p, 0, 256, ix->stream));
+  uint64_t launches = 1;
+  EPS_TRY(ensure_ell(ix, &launches));
+  if (ix->seed_rows_L != L) {  // contiguous copy of the query-independent seed rows
+    EPS_TRY(ix->s_seed_rows.reserve(static_cast<size_t>(L) * ix->dim * 4));
+    const int64_t tot = L * ix->dim;
+    gather_rows_kernel<<<static_cast<unsigned>((tot + 255) / 256), 256, 0, ix->stream>>>(
+        ix->d_vectors, ix->d_init_ids, static_cast<int>(L), dim, ix->s_seed_rows.as<float>());
+    EPS_CUDA(cudaGetLastError());
+    ix->seed_rows_L = L;
+    ++launches;
+  }
+  const int64_t seed_ld = (L + 3) & ~3ll;
+  EPS_TRY(ix->s_seed_dist.reserve(static_cast<size_t>(nq) * seed_ld * 4));
+  EPS_TRY(launch_distances(ix, ix->s_seed_rows.as<float>(), 0, L, d_queries, nq, ix->s_seed_dist.as<float>(), seed_ld,
+                           &launches));
+  GSArgs a;
+  a.vectors = ix->d_vectors; a.offsets = ix->d_offsets; a.nbrs = ix->d_nbrs; a.ell = ix->d_ell;
+  a.init_ids = ix->d_init_ids; a.seed_dist = ix->s_seed_dist.as<float>(); a.queries = d_queries;
+  a.vlog = vis.vlog; a.vlog_cap = vis.vlog_cap;
+  a.vset = vis.vset; a.vset_cap = vis.vset_cap; a.vset_max = vis.vset_max; a.vset_shift = vis.vset_shift;
+  a.visited = vis.visited; a.out_queue = d_queue;
+  a.work_counter = reinterpret_cast<int*>(ix->s_misc.as<unsigned char>() + 32);
+  a.stats = ix->s_misc.as<unsigned long long>();
+  a.visited_words = vis.words; a.seed_ld = seed_ld; a.dim = dim; a.metric = ix->metric;
+  a.vec4 = ix->vec4 ? 1 : 0; a.L = static_cast<int>(L); a.Lp = Lp; a.nq = static_cast<int>(nq);
+  a.W = width; a.R = R; a.slot_bytes = slot_bytes; a.fc = fc;
+  a.qtimes = nullptr;
+#ifdef EPS_GS_PROFILE
+  EPS_TRY(ix->s_tail.reserve(static_cast<size_t>(nq) * 32));  // borrowed scratch (the hybrid tail buffer is filled after the search)
+  a.qtimes = ix->s_tail.as<unsigned long long>();
+  ix->prof_nq = nq;
+#endif
+  // at most 4 resident CTAs per SM (what the auto rule picks for batches above one wave at 7 per SM, e.g. 1024 queries
+  // at L = 768): the register file has room for 128 registers per thread, so the instance that hardly spills runs;
+  // smaller batches keep 7 resident queries per SM
+  if (per_sm <= 4) graph_search_kernel<4><<<slots, kGsThreads, smem, ix->stream>>>(a);
+  else graph_search_kernel<7><<<slots, kGsThreads, smem, ix->stream>>>(a);
+  EPS_CUDA(cudaGetLastError());
+  if (stats) {
+    stats->n_seed += static_cast<uint64_t>(nq) * static_cast<uint64_t>(L);
+    stats->kernel_launches += launches;
+  }
+  return EPS_OK;
+}
+
+int prepare_visited(Index* ix, int slots, int64_t L, VisitedSets* v) {
   const int64_t words = ((ix->n_indexed + 31) / 32 + 3) & ~3ll;
   if (ix->visited_slots < slots || ix->s_visited.cap < static_cast<size_t>(slots) * words * 4) {
     EPS_TRY(ix->s_visited.reserve(static_cast<size_t>(slots) * words * 4));
@@ -902,54 +864,13 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
     ix->vset_clean_ptr = ix->s_vset.p;
     ix->vset_clean_cap = ix->s_vset.cap;
   }
-  EPS_TRY(ix->s_misc.reserve(256));  // [0..3] counters, [+32 B] work counter, [5] [30..31] developer hash-set counts,
-                                     // [8..24] developer phase timers, [25..29] developer prefix counts
-  EPS_CUDA(cudaMemsetAsync(ix->s_misc.p, 0, 256, ix->stream));
-  uint64_t launches = 1;
-  EPS_TRY(ensure_ell(ix, &launches));
-  if (ix->seed_rows_L != L) {  // contiguous copy of the query-independent seed rows
-    EPS_TRY(ix->s_seed_rows.reserve(static_cast<size_t>(L) * ix->dim * 4));
-    const int64_t tot = L * ix->dim;
-    gather_rows_kernel<<<static_cast<unsigned>((tot + 255) / 256), 256, 0, ix->stream>>>(
-        ix->d_vectors, ix->d_init_ids, static_cast<int>(L), dim, ix->s_seed_rows.as<float>());
-    EPS_CUDA(cudaGetLastError());
-    ix->seed_rows_L = L;
-    ++launches;
-  }
-  const int64_t seed_ld = (L + 3) & ~3ll;
-  EPS_TRY(ix->s_seed_dist.reserve(static_cast<size_t>(nq) * seed_ld * 4));
-  EPS_TRY(launch_distances(ix, ix->s_seed_rows.as<float>(), 0, L, d_queries, nq, ix->s_seed_dist.as<float>(), seed_ld,
-                           &launches));
-  GSArgs a;
-  a.vectors = ix->d_vectors; a.offsets = ix->d_offsets; a.nbrs = ix->d_nbrs; a.ell = ix->d_ell;
-  a.init_ids = ix->d_init_ids; a.seed_dist = ix->s_seed_dist.as<float>(); a.queries = d_queries;
+  // fresh ids of the running query in FIFO order: the migration to the bitmap and the bitmap reset read them
   constexpr int kVlogCap = 32768;
   EPS_TRY(ix->s_vlog.reserve(static_cast<size_t>(slots) * kVlogCap * 4));
-  a.vlog = ix->s_vlog.as<int32_t>(); a.vlog_cap = kVlogCap;
-  a.vset = ix->s_vset.as<uint32_t>(); a.vset_cap = vset_cap; a.vset_max = vset_cap / 4 * 3;
-  a.vset_shift = 32 - (__builtin_ctz(static_cast<unsigned>(vset_cap)) - 3);
-  a.visited = ix->s_visited.as<uint32_t>(); a.out_queue = d_queue;
-  a.work_counter = reinterpret_cast<int*>(ix->s_misc.as<unsigned char>() + 32);
-  a.stats = ix->s_misc.as<unsigned long long>();
-  a.visited_words = words; a.seed_ld = seed_ld; a.dim = dim; a.metric = ix->metric;
-  a.vec4 = ix->vec4 ? 1 : 0; a.L = static_cast<int>(L); a.Lp = Lp; a.nq = static_cast<int>(nq);
-  a.W = width; a.R = R; a.slot_bytes = slot_bytes; a.fc = fc;
-  a.qtimes = nullptr;
-#ifdef EPS_GS_PROFILE
-  EPS_TRY(ix->s_tail.reserve(static_cast<size_t>(nq) * 32));  // borrowed scratch (the hybrid tail buffer is filled after the search)
-  a.qtimes = ix->s_tail.as<unsigned long long>();
-  ix->prof_nq = nq;
-#endif
-  // at most 4 resident CTAs per SM (what the auto rule picks for batches above one wave at 7 per SM, e.g. 1024 queries
-  // at L = 768): the register file has room for 128 registers per thread, so the instance that hardly spills runs;
-  // smaller batches keep 7 resident queries per SM
-  if (per_sm <= 4) graph_search_kernel<4><<<slots, kGsThreads, smem, ix->stream>>>(a);
-  else graph_search_kernel<7><<<slots, kGsThreads, smem, ix->stream>>>(a);
-  EPS_CUDA(cudaGetLastError());
-  if (stats) {
-    stats->n_seed += static_cast<uint64_t>(nq) * static_cast<uint64_t>(L);
-    stats->kernel_launches += launches;
-  }
+  v->vset = ix->s_vset.as<uint32_t>(); v->vset_cap = vset_cap; v->vset_max = vset_cap / 4 * 3;
+  v->vset_shift = 32 - (__builtin_ctz(static_cast<unsigned>(vset_cap)) - 3);
+  v->visited = ix->s_visited.as<uint32_t>(); v->words = words;
+  v->vlog = ix->s_vlog.as<int32_t>(); v->vlog_cap = kVlogCap;
   return EPS_OK;
 }
 

@@ -80,6 +80,7 @@ struct Index {
   int64_t L_master = 500, L_local = 500;
   bool prefilter = false;
   bool force_brute = false;
+  int sparse_search = EPS_SPARSE_SEARCH_SCAN;  // sparse index: exact scan always, or the reference's graph branch
   int search_width = 1;          // candidates expanded per iteration (1 = the reference's sequential order)
   int graph_ring_slots = 0;      // row-ring slots per CTA of the graph kernel (0 = auto)
   int graph_ctas_per_sm = 0;     // cap on resident CTAs (= in-flight queries) per SM (0 = occupancy limit)
@@ -175,6 +176,11 @@ int sparse_append(Index* ix, int64_t first_row, int64_t n_rows, const int64_t* o
                   const float* values);
 int build_graph_sparse(Index* ix, int64_t n, const eps_build_params* params);
 
+// ---- sparse_graph.cu -----------------------------------------------------------------------
+// graph_search for sparse queries at width 1 (the reference's sequential order): d_queue [nq x L] sorted keys.
+int sparse_graph_search(Index* ix, const SparseQueries& q, int64_t nq, int64_t L, unsigned long long* d_queue,
+                        eps_stats* stats);
+
 // ---- graph_search.cu -----------------------------------------------------------------------
 // Best-first search of nq queries over the installed CSR graph with queue length L (<= n_indexed).
 // Output: d_queue [nq x L] sorted keys.
@@ -185,6 +191,18 @@ int ensure_ell(Index* ix, uint64_t* launches);  // fixed-stride adjacency of the
 // out[i] = row d_ids[i] of the table (contiguous copy; used for seed rows and for the build's repair searches)
 int gather_rows(Index* ix, const int32_t* d_ids, int64_t n, float* d_out);
 int read_graph_counters(Index* ix, eps_stats* stats);
+// Visited sets of `slots` concurrent graph queries at queue length L, shared by the dense and sparse kernels: per slot
+// an open-addressing hash set (all-ones = empty, refilled by the kernel), a bitmap of n_indexed bits for queries that
+// outgrow it (left zero by the kernel) and a log of the query's fresh ids.
+struct VisitedSets {
+  uint32_t* vset;
+  int vset_cap, vset_shift, vset_max;  // entries per slot, bucket shift, inserts before a query moves to the bitmap
+  uint32_t* visited;
+  int64_t words;                        // bitmap words per slot
+  int32_t* vlog;
+  int vlog_cap;
+};
+int prepare_visited(Index* ix, int slots, int64_t L, VisitedSets* v);
 
 // ---- finalize.cu ---------------------------------------------------------------------------
 // Post-filter walk / tail merge of VecSearchExecutor::Search (vec_search_executor.cpp:885-927).

@@ -202,9 +202,14 @@ def as_csr(rows):
             np.ascontiguousarray(values, np.float32))
 
 
+SPARSE_SEARCH_MODES = {"scan": 0, "graph": 1}
+
+
 class SparseIndex(Index):
-    """Device mirror of one sparse-vector field (eps_index_create_sparse): rows are appended as CSR, searches are
-    exact scans.  Config, deleted bits, attributes, string codes, facets, build and get_graph work as on Index."""
+    """Device mirror of one sparse-vector field (eps_index_create_sparse): rows are appended as CSR.  Searches are exact
+    scans by default; set_search_mode("graph") searches the graph that build() installed where the reference would
+    (n_indexed >= 512, no prefilter / force_brute), with the reference's results at IntraQueryThreads = 1.  Config,
+    deleted bits, attributes, string codes, facets, build and get_graph work as on Index."""
 
     def __init__(self, metric, dim, capacity=0, device=0):
         self.L = load_library()
@@ -231,6 +236,10 @@ class SparseIndex(Index):
     def rows(self):
         return int(self.L.eps_index_rows(self.h))
 
+    def set_search_mode(self, mode):
+        """"scan" (default): exact scan always; "graph": the reference's branch rule (eps_index_set_sparse_search)."""
+        check(self.L.eps_index_set_sparse_search(self.h, SPARSE_SEARCH_MODES.get(mode, mode)))
+
     def append(self, rows, first_row=None):
         """Append CSR rows (scipy CSR or (offsets, indices, values)) after the rows already mirrored."""
         off, idx, val = as_csr(rows)
@@ -238,7 +247,7 @@ class SparseIndex(Index):
         check(self.L.eps_index_append_sparse_rows(self.h, first, off.size - 1, _p(off), _p(idx), _p(val)))
 
     def search(self, queries, limit, filter_nodes=None, want_stats=True):
-        """Exact scan of CSR queries (eps_search_sparse_batch).  Returns ids [nq,limit], dists float64, counts, Stats."""
+        """Search of CSR queries (eps_search_sparse_batch), by the mode of set_search_mode.  Returns ids [nq,limit], dists float64, counts, Stats."""
         off, idx, val = as_csr(queries)
         nq = off.size - 1
         ids = np.empty((nq, limit), np.int64)

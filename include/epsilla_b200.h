@@ -177,10 +177,15 @@ EPS_API int eps_index_set_graph_tuning(eps_index* ix, int ring_slots, int ctas_p
  * 1 = wgmma TF32 on the fp32 rows (default), 2 = wgmma BF16 on a bf16 mirror of the table
  * (+50 % HBM).  Whatever the mode, the k' = k + max(118, k) best coarse candidates of every query are re-evaluated
  * with the exact fp32 direct form, so returned distances are fp32-exact, and a GUARD checks that no row outside
- * the candidate list can belong to the answer: with T = the k'-th best coarse distance, e_k = the exact k-th best
- * and E = the largest |coarse - exact| over the batch's own k' x nq re-scored rows, a query is safe when
- * e_k + 2 E <= T; unsafe queries are redone on the fp32 path (or, when many are unsafe, the batch is redone with a
- * 4x larger k' that the index remembers).  eps_stats.n_redone counts them.  The guard is on by default. */
+ * the candidate list can belong to the answer: with T = the k'-th best coarse distance, e_k = the exact k-th best,
+ * E = the largest |coarse - exact| over the batch's own k' x nq re-scored rows, M = the table's largest row norm and
+ * M_s = the largest norm among those re-scored rows, a query is safe when e_k + 2 E max(1, M / M_s) <= T; unsafe
+ * queries are redone on the fp32 path (or, when many are unsafe, the batch is redone with a 4x larger k' that the
+ * index remembers).  eps_stats.n_redone counts them.  The guard is on by default.
+ * What the guard assumes: a row's coarse error is at most the sampled E scaled by its norm relative to the sample's.
+ * The rule rests on sampled errors, not on a worst-case bound: rows of the same norm whose products cancel in a way
+ * none of the sampled rows does can still, in principle, escape it.  With the guard off the answer is the coarse
+ * candidate list re-scored, with no check. */
 EPS_API int eps_index_set_coarse(eps_index* ix, int mode);
 EPS_API int eps_index_set_coarse_guard(eps_index* ix, int on);
 

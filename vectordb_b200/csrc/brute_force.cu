@@ -378,7 +378,8 @@ __global__ void fill_keys_kernel(unsigned long long* p, int64_t n, unsigned long
 __global__ void __launch_bounds__(128) rescore_kernel(const float* __restrict__ vectors, int dim, int metric, int vec4,
                                                      const float* __restrict__ queries,
                                                      const unsigned long long* __restrict__ coarse, int kc, int kcp, int k,
-                                                     unsigned long long* __restrict__ out, unsigned* __restrict__ err_max_bits) {
+                                                     unsigned long long* __restrict__ out, unsigned* __restrict__ err_max_bits,
+                                                     const float* __restrict__ xnorm, unsigned* __restrict__ xn_max_bits) {
   extern __shared__ __align__(16) unsigned char rs_smem[];
   unsigned long long* keys = reinterpret_cast<unsigned long long*>(rs_smem);  // [kcp]
   float* qv = reinterpret_cast<float*>(keys + kcp);
@@ -394,7 +395,10 @@ __global__ void __launch_bounds__(128) rescore_kernel(const float* __restrict__ 
       const float d = warp_distance(metric, vec4 != 0, vectors + static_cast<int64_t>(id) * dim, qv, dim, lane);
       key = make_key(d, id);
       // calibration sample of the coarse pass: |coarse - exact| of a re-scored row (non-negative floats order as uints)
-      if (lane == 0 && err_max_bits) atomicMax(err_max_bits, __float_as_uint(fabsf(key_dist(ck) - d)));
+      if (lane == 0 && err_max_bits) {
+        atomicMax(err_max_bits, __float_as_uint(fabsf(key_dist(ck) - d)));
+        atomicMax(xn_max_bits, __float_as_uint(xnorm[id]));  // the sample's largest |x|^2
+      }
     }
     if (lane == 0) keys[c] = key;
   }
@@ -407,17 +411,24 @@ __global__ void __launch_bounds__(128) rescore_kernel(const float* __restrict__ 
 // Exactness guard of the coarse pass.  A row outside the coarse top-k' has coarse distance >= T (the k'-th best
 // coarse value); it can only belong to the exact top-k if its coarse error exceeds T - e_k (e_k = exact k-th best
 // after the re-score).  The batch's own re-scored rows (k' x nq samples of |coarse - exact|, whatever the operand
-// format or rounding mode did) calibrate the error: a query is SAFE when e_k + 2 * max|coarse - exact| <= T, or when
+// format or rounding mode did) calibrate the error E.  A coarse error grows with |x| |q|, and the sample only holds the
+// re-scored rows, so E is scaled by max(1, M / M_s), M = the table's largest |x| and M_s = the sample's: a row whose
+// norm is far above the candidates' cannot hide outside the list.  A query is SAFE when e_k + 2 * E_eff <= T, or when
 // fewer than k' rows exist at all.  Unsafe queries are redone (exact fp32 scan, or the whole batch with a larger k').
 // ------------------------------------------------------------------------------------------------
 __global__ void verify_exact_kernel(const unsigned long long* __restrict__ final_keys, int k_final, const float* __restrict__ thr,
-                                    const unsigned* __restrict__ err_max_bits, int nq, int* __restrict__ flags,
+                                    const unsigned* __restrict__ err_max_bits, const unsigned* __restrict__ xn_table_bits,
+                                    const unsigned* __restrict__ xn_sample_bits, int nq, int* __restrict__ flags,
                                     int* __restrict__ n_flagged) {
   const int q = blockIdx.x * blockDim.x + threadIdx.x;
   if (q >= nq) return;
   const unsigned long long kth = final_keys[static_cast<int64_t>(q) * k_final + (k_final - 1)];
   const float T = thr[q];
-  const float eps = 2.0f * __uint_as_float(*err_max_bits);
+  const float m2 = __uint_as_float(*xn_table_bits), s2 = __uint_as_float(*xn_sample_bits);  // squared norms
+  float err = __uint_as_float(*err_max_bits);
+  // s2 == 0 < m2: every re-scored row is zero and says nothing about the others (+inf: every such query is unsafe)
+  if (m2 > s2) err = s2 > 0.f ? err * sqrtf(m2 / s2) : INFINITY;
+  const float eps = 2.0f * err;
   const bool unsafe = (kth & kKeyMask) != kKeyInf && !isinf(T) && !(key_dist(kth) + eps <= T);
   flags[q] = unsafe ? 1 : 0;
   if (unsafe) atomicAdd(n_flagged, 1);
@@ -576,8 +587,8 @@ static int topk_impl(Index* ix, const float* d_queries, int64_t nq, int64_t row_
     EPS_TRY(ix->s_thr.reserve(static_cast<size_t>(nq) * 4));
     EPS_TRY(ix->s_cand.reserve(static_cast<size_t>(nq) * cand_cap * 8));
     EPS_TRY(ix->s_cand_cnt.reserve(static_cast<size_t>(nq + 4) * 4));
-    d_overflow = ix->s_cand_cnt.as<int>() + nq;  // [overflow, n_flagged, err_max bits]
-    EPS_CUDA(cudaMemsetAsync(d_overflow, 0, 12, ix->stream));
+    d_overflow = ix->s_cand_cnt.as<int>() + nq;  // [overflow, n_flagged, err_max bits, sample's max |x|^2 bits]
+    EPS_CUDA(cudaMemsetAsync(d_overflow, 0, 16, ix->stream));
   }
   for (int64_t c0 = 0; c0 < n;) {
     // Chunk 0 (and every chunk of the SIMT path) materialises the [nq x chunk] distance tile and selects from
@@ -630,7 +641,8 @@ static int topk_impl(Index* ix, const float* d_queries, int64_t nq, int64_t row_
     unsigned* d_err = reinterpret_cast<unsigned*>(d_overflow + 2);
     rescore_kernel<<<static_cast<unsigned>(nq), 128, rs_smem, ix->stream>>>(ix->d_vectors, static_cast<int>(ix->dim), ix->metric,
                                                                           ix->vec4 ? 1 : 0, d_queries, d_topk, kc, kcp,
-                                                                          static_cast<int>(k_final), d_final, d_err);
+                                                                          static_cast<int>(k_final), d_final, d_err,
+                                                                          ix->s_xnorm.as<float>(), d_err + 1);
     EPS_CUDA(cudaGetLastError());
     ++launches;
     std::vector<int> h_flags;
@@ -639,7 +651,8 @@ static int topk_impl(Index* ix, const float* d_queries, int64_t nq, int64_t row_
     if (guard) {
       EPS_TRY(ix->s_flags.reserve(static_cast<size_t>(nq) * 4));
       verify_exact_kernel<<<static_cast<unsigned>((nq + 127) / 128), 128, 0, ix->stream>>>(
-          d_final, static_cast<int>(k_final), ix->s_thr.as<float>(), d_err, static_cast<int>(nq), ix->s_flags.as<int>(), d_overflow + 1);
+          d_final, static_cast<int>(k_final), ix->s_thr.as<float>(), d_err, ix->s_xnorm_max.as<unsigned>(), d_err + 1,
+          static_cast<int>(nq), ix->s_flags.as<int>(), d_overflow + 1);
       EPS_CUDA(cudaGetLastError());
       ++launches;
       h_flags.resize(static_cast<size_t>(nq));

@@ -453,7 +453,7 @@ void eps_index_destroy(eps_index* h) {
   }
   eps::DevBuf* bufs[] = {&ix->s_queries, &ix->s_dist, &ix->s_topk, &ix->s_topk2, &ix->s_pass, &ix->s_filter,
                          &ix->s_vset, &ix->s_visited, &ix->s_vlog, &ix->s_queue, &ix->s_tail, &ix->s_out_ids, &ix->s_out_dists,
-                         &ix->s_out_counts, &ix->s_stats, &ix->s_misc, &ix->s_seed_rows, &ix->s_seed_dist, &ix->s_xnorm, &ix->s_qnorm, &ix->s_coarse, &ix->s_thr, &ix->s_cand, &ix->s_cand_cnt, &ix->s_bf16, &ix->s_qbf16, &ix->s_flags, &ix->s_sparse_q};
+                         &ix->s_out_counts, &ix->s_stats, &ix->s_misc, &ix->s_seed_rows, &ix->s_seed_dist, &ix->s_xnorm, &ix->s_qnorm, &ix->s_coarse, &ix->s_thr, &ix->s_cand, &ix->s_cand_cnt, &ix->s_bf16, &ix->s_qbf16, &ix->s_flags, &ix->s_sparse_q, &ix->s_xnorm_max};
   for (auto* b : bufs) b->release();
   if (ix->h_out) cudaFreeHost(ix->h_out);
   for (auto& ev : ix->ev) if (ev) cudaEventDestroy(ev);

@@ -92,13 +92,13 @@ struct Index {
   // scratch
   DevBuf s_queries, s_dist, s_topk, s_topk2, s_pass, s_filter, s_vset, s_visited, s_vlog, s_queue, s_tail, s_out_ids, s_out_dists,
       s_out_counts, s_stats, s_misc, s_seed_rows, s_seed_dist, s_xnorm, s_qnorm, s_coarse, s_thr, s_cand, s_cand_cnt, s_bf16, s_qbf16, s_flags,
-      s_sparse_q;
+      s_sparse_q, s_xnorm_max;
   int coarse_mode = 1;           // exact-scan coarse pass: 0 = fp32 SIMT only, 1 = wgmma TF32, 2 = wgmma bf16 mirror
   int coarse_guard = 1;          // verify the coarse pass after the re-score and redo unsafe queries (brute_force.cu)
   int coarse_boost = 1;          // multiplier of k' learnt by the guard for this table (1, 4, 16, 64)
   int64_t bf16_rows = 0;
   const void* bf16_ptr = nullptr;
-  int64_t xnorm_rows = 0;        // rows whose |x|^2 is current in s_xnorm
+  int64_t xnorm_rows = 0;        // rows whose |x|^2 is current in s_xnorm; s_xnorm_max holds the largest (float bits)
   const void* xnorm_ptr = nullptr;
   int64_t visited_slots = 0;
   const void* vis_clean_ptr = nullptr;  // geometry for which the visited bitmaps are known to be zero

@@ -380,8 +380,10 @@ __global__ void __launch_bounds__(kTcThreads, 1) tc_dist_kernel(const __grid_con
   }
 }
 
-// |x|^2 per row (fp32, warp per row) for the L2 expansion of the coarse pass.
-__global__ void row_norm_kernel(const float* __restrict__ v, int64_t row0, int64_t n, int dim, float* __restrict__ out) {
+// |x|^2 per row (fp32, warp per row) for the L2 expansion of the coarse pass and the guard's norm ratio; with max_bits
+// set, also the largest |x|^2 seen (non-negative floats order as their bits).
+__global__ void row_norm_kernel(const float* __restrict__ v, int64_t row0, int64_t n, int dim, float* __restrict__ out,
+                                unsigned* __restrict__ max_bits = nullptr) {
   const int64_t w = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (w >= n) return;
@@ -389,7 +391,10 @@ __global__ void row_norm_kernel(const float* __restrict__ v, int64_t row0, int64
   float s = 0.f;
   for (int i = lane; i < dim; i += 32) s = fmaf(p[i], p[i], s);
   s = warp_sum(s);
-  if (lane == 0) out[row0 + w] = s;
+  if (lane == 0) {
+    out[row0 + w] = s;
+    if (max_bits && s >= 0.f) atomicMax(max_bits, __float_as_uint(s));
+  }
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -458,16 +463,19 @@ int tc_launch_distances(Index* ix, int64_t row_start, int64_t n, const float* d_
                         int64_t ldd, uint64_t* launches, const TcFused* fused) {
   const int dim = static_cast<int>(ix->dim);
   const bool bf16 = ix->coarse_mode == 2;
+  // |x|^2 of every row and the table's largest (every metric: the guard scales its error sample by the norm ratio)
+  if (ix->xnorm_rows < ix->n_rows) {  // row norms for rows appended since the last call
+    EPS_TRY(ix->s_xnorm.reserve(static_cast<size_t>(ix->capacity > ix->n_rows ? ix->capacity : ix->n_rows) * 4));
+    EPS_TRY(ix->s_xnorm_max.reserve(4));
+    if (ix->s_xnorm.p != ix->xnorm_ptr) { ix->xnorm_rows = 0; ix->xnorm_ptr = ix->s_xnorm.p; }
+    if (ix->xnorm_rows == 0) EPS_CUDA(cudaMemsetAsync(ix->s_xnorm_max.p, 0, 4, ix->stream));
+    const int64_t cnt = ix->n_rows - ix->xnorm_rows;
+    row_norm_kernel<<<static_cast<unsigned>((cnt * 32 + 255) / 256), 256, 0, ix->stream>>>(
+        ix->d_vectors, ix->xnorm_rows, cnt, dim, ix->s_xnorm.as<float>(), ix->s_xnorm_max.as<unsigned>());
+    ix->xnorm_rows = ix->n_rows;
+    ++*launches;
+  }
   if (ix->metric == EPS_METRIC_L2) {
-    if (ix->xnorm_rows < ix->n_rows) {  // row norms for rows appended since the last call
-      EPS_TRY(ix->s_xnorm.reserve(static_cast<size_t>(ix->capacity > ix->n_rows ? ix->capacity : ix->n_rows) * 4));
-      if (ix->s_xnorm.p != ix->xnorm_ptr) { ix->xnorm_rows = 0; ix->xnorm_ptr = ix->s_xnorm.p; }
-      const int64_t cnt = ix->n_rows - ix->xnorm_rows;
-      row_norm_kernel<<<static_cast<unsigned>((cnt * 32 + 255) / 256), 256, 0, ix->stream>>>(ix->d_vectors, ix->xnorm_rows, cnt,
-                                                                                            dim, ix->s_xnorm.as<float>());
-      ix->xnorm_rows = ix->n_rows;
-      ++*launches;
-    }
     EPS_TRY(ix->s_qnorm.reserve(static_cast<size_t>(nq) * 4));
     row_norm_kernel<<<static_cast<unsigned>((nq * 32 + 255) / 256), 256, 0, ix->stream>>>(d_queries, 0, nq, dim,
                                                                                          ix->s_qnorm.as<float>());

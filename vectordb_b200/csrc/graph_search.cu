@@ -35,10 +35,15 @@
 //     its run; that bitmap is cleared after the query — on large tables only the words the query touched, from a log
 //     of its fresh ids.
 // every iteration picks up to W (the search width) unchecked candidates, and the next pick waits until all their rows
-//   are consumed and merged.  Width 1 has the visit order, results and distance-evaluation counts of the reference
-//   at IntraQueryThreads = 1; widths 2..8 expand W candidates together — the device analogue of IntraQueryThreads > 1,
-//   not bit-identical to the sequential order but, unlike that racy mode, the same on every run: the queue after a
-//   merge is the best L of the queue and all fresh rows, whatever order the rows land in.
+//   are consumed and merged.  The result at any width W is that of this rule: each step takes the first
+//   min(W, #unchecked) unchecked queue entries and marks them checked, tests-and-sets every id of their full CSR rows
+//   against one visited set, evaluates the fresh ids, and keeps the best L by (distance, id) of the queue and the fresh
+//   rows, checked flags kept; the search stops when nothing is unchecked.  It holds because at a pick the pending buffer
+//   is empty, continuation chunks are drained before the next pick, and keys accepted against a stale bound are evicted
+//   by the merge, so neither the landing order of rows nor the launch geometry can change it.  Width 1 is the reference
+//   at IntraQueryThreads = 1 (visit order, results, distance-evaluation counts); widths 2..8 are the device analogue of
+//   IntraQueryThreads > 1, deterministic where that mode races.  tests/graph_model.py restates the rule and
+//   tests/test_gpu_graph_exact.py holds the kernel to it bit for bit.
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>

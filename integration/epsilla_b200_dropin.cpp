@@ -474,6 +474,8 @@ void ANNGraphSegment::BuildFromVectorTable(VectorColumnData vector_column, int64
     if (eps_index_create(&ix, metric, dim, table, n, b200::DeviceOrdinal()) != EPS_OK) die("create");
     if (eps_index_sync_rows(ix, n) != EPS_OK) die("sync_rows");
   }
+  // this index only builds the graph that the mirror installs: no screen sketch for it
+  if (eps_index_set_graph_screen(ix, EPS_GRAPH_SCREEN_OFF) != EPS_OK) die("set_graph_screen");
   if (eps_index_build(ix, n, nullptr) != EPS_OK) die("build");
   int64_t ni = 0, ne = 0, nav = 0;
   if (eps_index_get_graph(ix, &ni, &ne, nullptr, nullptr, &nav) != EPS_OK) die("get_graph");

@@ -215,6 +215,7 @@ int install_csr(Index* ix, int64_t n, const int64_t* off, const int32_t* nb, int
   if (ix->d_nbrs) { cudaFree(ix->d_nbrs); ix->d_nbrs = nullptr; }
   if (ix->d_init_ids) { cudaFree(ix->d_init_ids); ix->d_init_ids = nullptr; }
   if (ix->d_ell) { cudaFree(ix->d_ell); ix->d_ell = nullptr; }
+  free_sketch(ix);
   ix->seed_rows_L = 0;
   ix->init_L = 0;
   ix->n_indexed = 0;

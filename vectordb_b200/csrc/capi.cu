@@ -140,6 +140,7 @@ static void free_graph(Index* ix) {
   if (ix->d_init_ids) cudaFree(ix->d_init_ids);
   if (ix->d_ell) cudaFree(ix->d_ell);
   ix->d_ell = nullptr;
+  free_sketch(ix);
   ix->seed_rows_L = 0;
   ix->d_offsets = nullptr;
   ix->d_nbrs = nullptr;
@@ -436,6 +437,7 @@ void eps_index_destroy(eps_index* h) {
       v->view_of = nullptr; v->detached_view = true;
       v->d_vectors = nullptr; v->n_rows = 0; v->capacity = 0;
       v->d_offsets = nullptr; v->d_nbrs = nullptr; v->d_ell = nullptr; v->n_indexed = 0; v->n_edges = 0;
+      eps::free_sketch(v);
       v->d_deleted = nullptr; v->deleted_bytes = 0; v->any_deleted = false;
       v->d_attrs = nullptr; v->attr_rows = 0;
       v->d_sp_ptr = nullptr; v->d_sp_elems = nullptr; v->d_sp_norm2 = nullptr; v->sp_nnz = 0;
@@ -453,9 +455,11 @@ void eps_index_destroy(eps_index* h) {
   }
   eps::DevBuf* bufs[] = {&ix->s_queries, &ix->s_dist, &ix->s_topk, &ix->s_topk2, &ix->s_pass, &ix->s_filter,
                          &ix->s_vset, &ix->s_visited, &ix->s_vlog, &ix->s_queue, &ix->s_tail, &ix->s_out_ids, &ix->s_out_dists,
-                         &ix->s_out_counts, &ix->s_stats, &ix->s_misc, &ix->s_seed_rows, &ix->s_seed_dist, &ix->s_xnorm, &ix->s_qnorm, &ix->s_coarse, &ix->s_thr, &ix->s_cand, &ix->s_cand_cnt, &ix->s_bf16, &ix->s_qbf16, &ix->s_flags, &ix->s_sparse_q, &ix->s_xnorm_max};
+                         &ix->s_out_counts, &ix->s_stats, &ix->s_misc, &ix->s_seed_rows, &ix->s_seed_dist, &ix->s_xnorm, &ix->s_qnorm, &ix->s_coarse, &ix->s_thr, &ix->s_cand, &ix->s_cand_cnt, &ix->s_bf16, &ix->s_qbf16, &ix->s_flags, &ix->s_sparse_q, &ix->s_xnorm_max,
+                         &ix->s_qsk};
   for (auto* b : bufs) b->release();
   if (ix->h_out) cudaFreeHost(ix->h_out);
+  if (ix->d_screened) cudaFree(ix->d_screened);
   for (auto& ev : ix->ev) if (ev) cudaEventDestroy(ev);
   cudaStreamDestroy(ix->stream);
   delete ix;
@@ -491,6 +495,8 @@ int eps_index_create_view(eps_index* base_h, eps_index** out) {
   ix->search_width = base->search_width; ix->sparse_search = base->sparse_search; ix->graph_ring_slots = base->graph_ring_slots;
   ix->graph_ctas_per_sm = base->graph_ctas_per_sm; ix->num_sms = base->num_sms;
   ix->coarse_mode = base->coarse_mode; ix->coarse_guard = base->coarse_guard; ix->coarse_boost = base->coarse_boost;
+  ix->graph_screen = base->graph_screen; ix->sk_m = base->sk_m; ix->sk_share = base->sk_share; ix->sk_g = base->sk_g;
+  ix->sk_scale = base->sk_scale; ix->sk_eps = base->sk_eps; ix->d_sk_basis = base->d_sk_basis; ix->d_sk = base->d_sk;
   cudaError_t e = cudaStreamCreateWithFlags(&ix->stream, cudaStreamNonBlocking);
   if (e != cudaSuccess) { delete ix; return eps::fail(EPS_ERR_CUDA, cudaGetErrorString(e)); }
   for (auto& ev : ix->ev) cudaEventCreate(&ev);
@@ -538,6 +544,7 @@ int eps_index_adopt_device_rows(eps_index* h, const float* d_vectors, int64_t n_
   ix->d_vectors = const_cast<float*>(d_vectors);
   // state derived from the previous table: gathered seed rows always, the graph itself if it no longer fits
   ix->seed_rows_L = 0;
+  eps::free_sketch(ix);  // computed from the rows this call replaces
   if (ix->n_indexed > n_rows) eps::free_graph(ix);
   ix->n_rows = n_rows;
   if (n_rows > ix->capacity) ix->capacity = n_rows;
@@ -590,6 +597,7 @@ int eps_index_set_graph(eps_index* h, int64_t n_indexed, const int64_t* offsets,
   ix->n_indexed = n_indexed;
   ix->n_edges = e;
   ix->nav = nav;
+  eps::ensure_sketch(ix);
   return EPS_OK;
 }
 
@@ -599,7 +607,9 @@ int eps_index_build(eps_index* h, int64_t n, const eps_build_params* params) {
   EPS_TRY(eps::check_device(ix->device));
   EPS_TRY(check_mutable(ix));
   if (ix->sparse) return eps::build_graph_sparse(ix, n, params);
-  return eps::build_graph(ix, n, params);
+  EPS_TRY(eps::build_graph(ix, n, params));
+  eps::ensure_sketch(ix);
+  return EPS_OK;
 }
 
 int eps_index_get_graph(eps_index* h, int64_t* n_indexed, int64_t* n_edges, int64_t* offsets, int64_t* nbrs,
@@ -955,6 +965,37 @@ int eps_index_set_graph_tuning(eps_index* h, int ring_slots, int ctas_per_sm) {
     return eps::fail(EPS_ERR_INVALID_ARGUMENT, "ring_slots must be in [0, 24] and ctas_per_sm in [0, 32] (0 = auto)");
   ix->graph_ring_slots = ring_slots;
   ix->graph_ctas_per_sm = ctas_per_sm;
+  return EPS_OK;
+}
+
+int eps_index_set_graph_screen(eps_index* h, int mode) {
+  Index* ix = reinterpret_cast<Index*>(h);
+  if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");
+  EPS_TRY(eps::dense_only(ix));
+  EPS_TRY(check_mutable(ix));
+  if (mode != EPS_GRAPH_SCREEN_OFF && mode != EPS_GRAPH_SCREEN_ON && mode != EPS_GRAPH_SCREEN_AUTO)
+    return eps::fail(EPS_ERR_INVALID_ARGUMENT, "graph screen mode must be 0 (off), 1 (on) or 2 (auto)");
+  EPS_TRY(eps::check_device(ix->device));
+  ix->graph_screen = mode;
+  eps::ensure_sketch(ix);
+  return EPS_OK;
+}
+
+int eps_index_graph_screen_info(eps_index* h, int* active, double* share, uint64_t* n_screened) {
+  Index* ix = reinterpret_cast<Index*>(h);
+  if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");
+  if (active) *active = eps::screen_on(ix) ? 1 : 0;
+  if (share) *share = ix->sk_share;
+  if (n_screened) {
+    *n_screened = 0;
+    if (ix->d_screened) {
+      EPS_TRY(eps::check_device(ix->device));
+      EPS_CUDA(cudaStreamSynchronize(ix->stream));
+      unsigned long long v = 0;
+      EPS_CUDA(cudaMemcpy(&v, ix->d_screened, 8, cudaMemcpyDeviceToHost));
+      *n_screened = v;
+    }
+  }
   return EPS_OK;
 }
 

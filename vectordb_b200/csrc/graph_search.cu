@@ -34,6 +34,9 @@
 //     query that would fill the set beyond 3/4 moves to a bitmap of n bits (atomicOr test-and-set) for the rest of
 //     its run; that bitmap is cleared after the query — on large tables only the words the query touched, from a log
 //     of its fresh ids.
+//   * screen (L2, sketch.cu): once the queue holds L entries, the fresh ids of a step are checked against a proven lower
+//     bound from 32-float principal-subspace sketches of the row and the query, and only those it cannot reject enter
+//     the FIFO and have their rows fetched (screen_fresh; DESIGN.md §K2);
 // every iteration picks up to W (the search width) unchecked candidates, and the next pick waits until all their rows
 //   are consumed and merged.  The result at any width W is that of this rule: each step takes the first
 //   min(W, #unchecked) unchecked queue entries and marks them checked, tests-and-sets every id of their full CSR rows
@@ -45,6 +48,7 @@
 //   IntraQueryThreads > 1, deterministic where that mode races.  tests/graph_model.py restates the rule and
 //   tests/test_gpu_graph_exact.py holds the kernel to it bit for bit.
 #include <algorithm>
+#include <cfloat>
 #include <cstdio>
 #include <cstdlib>
 
@@ -62,7 +66,7 @@ constexpr int kRounds = kMaxW * kEll / kGsThreads;  // adjacency slots per threa
 
 // Developer build only (make EXTRA=-DEPS_GS_PROFILE): per-phase cycle counters of warp 0 (pick / adjacency / merge /
 // barrier waits) and of warp 1 (row wait / row math), summed over CTAs into stats[8..23], and the prefix-rejection
-// counts of prof_prefix_fails in stats[25..29].  Compiled out otherwise.
+// counts of prof_prefix_fails in stats[25..29] and of prof_sketch_fails in stats[32..33].  Compiled out otherwise.
 #ifdef EPS_GS_PROFILE
 #define GS_T(var) const long long var = clock64()
 #define GS_ACC(slot, t0, t1) do { if (lane == 0) prof[slot] += (t1) - (t0); } while (0)
@@ -99,6 +103,16 @@ struct GSArgs {
   int fc;                         // fresh-id FIFO capacity (power of two)
   unsigned long long* qtimes;     // developer build: [nq x 2] globaltimer at query start / end (null otherwise)
   int slot_bytes;                 // ring slot pitch (row bytes, multiple of 16); 0 when rows are not staged
+  // screen (sketch.cu; sk == null: off): fresh neighbours whose sketch bound fails the bound never enter the FIFO
+  const float* sk;                // [n x kSketch] row sketches, then [n] their error bounds
+  const float* qsk;               // [nq x kSketch] query sketches, then [nq] their error bounds
+  int64_t n_sk;                   // rows sketched (n_indexed)
+  float sk_g, sk_scale;           // rounded-down factors of the bound (see screen_fresh)
+  unsigned long long* n_screened; // ids the screen dropped, summed over every search of the handle
+#ifdef EPS_GS_PROFILE
+  const float* prof_basis;        // [prof_m x dim] principal subspace of the table (null: not counted)
+  int prof_m;
+#endif
 };
 
 template <bool L2>
@@ -180,7 +194,101 @@ __device__ __forceinline__ void prof_prefix_fails(const unsigned char* first, ui
     }
   }
 }
+
+// Developer build: could a lower bound from the table's principal subspace reject a staged L2 row before the row is
+// read?  P [m x dim4 float4] has orthonormal rows (sketch.cu), so |P(x - q)|^2 <= |x - q|^2; cnt[0] / cnt[1] count the
+// rows for which the bound of the first 32 / all m rows of P, shrunk by 1e-3 to cover the rounding of both sides
+// (a bound held to the kernel's fp32 sum needs about 1e-4 at d = 768), already fails the bound of the consumer.
+template <int S>
+__device__ __forceinline__ void prof_sketch_fails(const unsigned char* first, uint32_t step, unsigned mask, const float4* q, int dim4,
+                                                  int lane, const int* slot_id, int cw, unsigned long long bound,
+                                                  const float4* __restrict__ P, int m, unsigned long long* cnt) {
+  float acc[S];
+#pragma unroll
+  for (int s = 0; s < S; ++s) acc[s] = 0.f;
+  for (int j = 0; j < m; ++j) {
+    float part[S];
+#pragma unroll
+    for (int s = 0; s < S; ++s) part[s] = 0.f;
+    for (int c = lane; c < dim4; c += 32) {
+      const float4 p = __ldg(P + static_cast<size_t>(j) * dim4 + c), y = q[c];
+#pragma unroll
+      for (int s = 0; s < S; ++s)
+        if ((mask >> s) & 1u) {
+          const float4 x = reinterpret_cast<const float4*>(first + s * step)[c];
+          part[s] += p.x * (x.x - y.x) + p.y * (x.y - y.y) + p.z * (x.z - y.z) + p.w * (x.w - y.w);
+        }
+    }
+#pragma unroll
+    for (int s = 0; s < S; ++s) {
+      const float v = warp_sum(part[s]);
+      acc[s] = fmaf(v, v, acc[s]);
+    }
+    if (j == 31 || j == m - 1) {
+#pragma unroll
+      for (int s = 0; s < S; ++s)
+        if (lane == s && ((mask >> s) & 1u) &&
+            make_key(acc[s] * (1.f - 1e-3f), static_cast<uint32_t>(slot_id[cw + 3 * s])) >= bound)
+          ++cnt[j == m - 1 ? 1 : 0];
+    }
+  }
+}
 #endif
+
+// Screen of the fresh ids fifo[tail .. tail + total) of one expansion step (all 128 threads).  Eight lanes per id read its
+// sketch s_x (one float4 each) and its error bound ex_x; the loads of up to kScreenIds ids are issued before any is
+// used.  With p_q, E_q the query's sketch and bound (shared memory) and l^ = the fp32 sum of (s_x - p_q)^2:
+//   LB = [(sqrt(l^ (1 - gamma_{m+2})) - ex_x - E_q)+]^2 (1 - 2 (d + 2) 2^-24) / (1 + eps),   every step rounded down.
+// |s_x - p_q| - ex_x - E_q <= |P~(x - q)| <= sqrt(1 + eps) |x - q|, and the kernel's fp32 L2 sum of the row is at least
+// (1 - 2 (d + 2) 2^-24) |x - q|^2, so LB never exceeds the distance the consumer would compute.  An id is dropped iff
+// make_key(LB, id) >= bound; the consumer's bound is at most this one, so it would have dropped the id too.  Bit i of
+// keep is set for every id i that stays.
+constexpr int kScreenIds = 64;  // ids whose loads are in flight together (4 per 8-lane group)
+__device__ __forceinline__ void screen_fresh(const GSArgs& a, const int* fifo, unsigned fmask, uint32_t tail, int total, const float* psk,
+                                             unsigned long long bound, int tid, unsigned* keep) {
+  const int g = tid >> 3, j = tid & 7;
+  constexpr int kPer = kScreenIds / (kGsThreads / 8);
+  const float4* sk4 = reinterpret_cast<const float4*>(a.sk);
+  const float* skex = a.sk + a.n_sk * kSketch;
+  const float4 p0 = reinterpret_cast<const float4*>(psk)[j];
+  const float eq = psk[kSketch];
+  for (int i0 = 0; i0 < total; i0 += kScreenIds) {
+    int id[kPer];
+    float4 x0[kPer];
+    float xe[kPer];
+#pragma unroll
+    for (int b = 0; b < kPer; ++b) {
+      const int i = i0 + b * (kGsThreads / 8) + g;
+      id[b] = i < total ? fifo[(tail + static_cast<uint32_t>(i)) & fmask] : -1;
+      x0[b] = p0;
+      xe[b] = 0.f;
+      if (id[b] >= 0) {
+        x0[b] = __ldg(sk4 + static_cast<int64_t>(id[b]) * (kSketch / 4) + j);
+        if (j == 0) xe[b] = __ldg(skex + id[b]);
+      }
+    }
+#pragma unroll
+    for (int b = 0; b < kPer; ++b) {
+      float acc = 0.f, d;
+      d = x0[b].x - p0.x; acc = fmaf(d, d, acc); d = x0[b].y - p0.y; acc = fmaf(d, d, acc);
+      d = x0[b].z - p0.z; acc = fmaf(d, d, acc); d = x0[b].w - p0.w; acc = fmaf(d, d, acc);
+      acc += __shfl_xor_sync(kFull, acc, 1);
+      acc += __shfl_xor_sync(kFull, acc, 2);
+      acc += __shfl_xor_sync(kFull, acc, 4);
+      if (j == 0 && id[b] >= 0) {
+        const int i = i0 + b * (kGsThreads / 8) + g;
+        float r = __fsqrt_rd(__fmul_rd(acc, a.sk_g));
+        r = __fsub_rd(__fsub_rd(r, xe[b]), eq);
+        bool drop = false;
+        if (r > 0.f) {  // false for NaN as well
+          const float lb = __fmul_rd(__fmul_rd(r, r), a.sk_scale);
+          drop = lb <= FLT_MAX && make_key(lb, static_cast<uint32_t>(id[b])) >= bound;
+        }
+        if (!drop) atomicOr(keep + (i >> 5), 1u << (i & 31));
+      }
+    }
+  }
+}
 
 // Consumer step of one warp over its S slots (slot of local index s = cw + 3 s): wait for the landed rows, distances,
 // accepted keys to the pending buffer.  Returns nothing; the caller refills the slots.
@@ -201,6 +309,9 @@ __device__ __forceinline__ void consume_slots(const GSArgs& a, unsigned occ_mask
 #ifdef EPS_GS_PROFILE
     if (a.metric == EPS_METRIC_L2)
       prof_prefix_fails<S>(first, step, occ_mask, reinterpret_cast<const float4*>(qv), a.dim >> 2, lane, slot_id, cw, bound, prefix_cnt);
+    if (a.metric == EPS_METRIC_L2 && a.prof_basis)
+      prof_sketch_fails<S>(first, step, occ_mask, reinterpret_cast<const float4*>(qv), a.dim >> 2, lane, slot_id, cw, bound,
+                           reinterpret_cast<const float4*>(a.prof_basis), a.prof_m, prefix_cnt + 5);
 #endif
   } else {
     const float* rows[S];
@@ -221,8 +332,9 @@ __device__ __forceinline__ void consume_slots(const GSArgs& a, unsigned occ_mask
 
 // Two register budgets of the same kernel: 72 registers per thread allow 7 resident CTAs per SM but spill 376 B per
 // thread to local memory (348 B of spill loads); 128 registers allow 4 and spill 12 B (16 B of loads).  graph_search
-// picks the instance from the geometry it launches.
-template <int kMinCtas>
+// picks the instance from the geometry it launches.  kScreen: the screen is compiled in only where it runs, so that a
+// search without it (other metrics, tables it cannot pay on) keeps the registers of the kernel without it.
+template <int kMinCtas, bool kScreen>
 __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSArgs a) {
   extern __shared__ __align__(128) unsigned char gs_smem[];
   const int dim4p = (a.dim + 3) & ~3;
@@ -232,7 +344,8 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
   unsigned long long* cs = pend + kPC;                                                             // [kPC]
   unsigned long long* bars = cs + kPC;                                                             // [kMaxR]
   float* qv = reinterpret_cast<float*>(bars + kMaxR);                                              // [dim4p]
-  int* pos = reinterpret_cast<int*>(qv + dim4p);                                                   // [kPC]
+  float* psk = qv + dim4p;                                                                         // [kSketch + 4] query sketch, bound (screen)
+  int* pos = reinterpret_cast<int*>(psk + (kScreen ? kSketch + 4 : 0));                            // [kPC]
   int* fifo = pos + kPC;                                                                           // [fc]
   int* slot_id = fifo + a.fc;                                                                      // [kMaxR] row id in each ring slot
   unsigned* ubits = reinterpret_cast<unsigned*>(slot_id + kMaxR);                                  // [(Lp + 31) / 32] unchecked-entry bitmap
@@ -241,6 +354,7 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
   __shared__ int s_cid[kMaxW];
   __shared__ int s_wcnt[kRounds][kGsThreads / 32];
   __shared__ long long s_cont_e[kMaxW], s_cont_end[kMaxW];
+  __shared__ unsigned s_keep[kMaxW * kEll / 32];  // screen: bit i = fresh id i of the step stays
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   // warp 0 picks candidates and leads the adjacency step; warps 1-3 are the row consumers: ring slot s belongs to
@@ -266,11 +380,13 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
   // barrier guards a slot.  Per-slot state (occupied, mbarrier phase parity) is a pair of warp-uniform bit masks.
   unsigned occ_mask = 0u, par_mask = 0u;
   const int n_own = cw >= 0 ? (R - cw + 2) / 3 : 0;  // slots cw, cw + 3, ... < R
-  unsigned long long st_ndist = 0, st_nexp = 0, st_nedge = 0;
+  unsigned long long st_ndist = 0, st_nexp = 0, st_nedge = 0, st_nscr = 0;
 #ifdef EPS_GS_PROFILE
   long long prof[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // 0 barrier X, 1 merge, 2 row wait, 3 row math, 4 pick, 5 barrier 1, 6 adjacency+visited, 7 barrier 2 + FIFO
   const long long t_kernel0 = clock64();
-  unsigned long long prefix_cnt[5] = {0, 0, 0, 0, 0};  // staged L2 rows evaluated; of them, rows whose 1/4 .. 4/4 prefix fails the bound
+  // staged L2 rows evaluated; of them, rows whose 1/4 .. 4/4 prefix fails the bound; rows whose 32- / m-float sketch
+  // bound fails it
+  unsigned long long prefix_cnt[7] = {0, 0, 0, 0, 0, 0, 0};
   unsigned long long prof_vtest = 0, prof_migrated = 0;  // hash-set test-and-inserts of this thread; queries moved to the bitmap
 #else
   unsigned long long* prefix_cnt = nullptr;
@@ -291,6 +407,8 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
     // ---- seed (InitializeSetLPara): precomputed distances of the query-independent seed set ----
     for (int i = tid; i < a.dim; i += kGsThreads) qv[i] = a.queries[static_cast<int64_t>(q) * a.dim + i];
     for (int i = a.dim + tid; i < dim4p; i += kGsThreads) qv[i] = 0.f;
+    if (kScreen && tid <= kSketch)
+      psk[tid] = tid < kSketch ? a.qsk[static_cast<int64_t>(q) * kSketch + tid] : a.qsk[static_cast<int64_t>(a.nq) * kSketch + q];
     bool hashed = L <= a.vset_max;  // the visited set is the hash set (false: the query has moved to the bitmap)
     for (int i = tid; i < a.Lp; i += kGsThreads) {
       unsigned long long key = kKeyInf;
@@ -314,7 +432,9 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
     for (int w = tid; w < ((L + 31) >> 5); w += kGsThreads)  // every seed starts unchecked
       ubits[w] = (w * 32 + 32 <= L) ? 0xffffffffu : ((1u << (L & 31)) - 1u);
     if (tid == 0) st_ndist += static_cast<unsigned long long>(L);
-    uint32_t fifo_tail = 0;
+    uint32_t fifo_tail = 0;   // ids appended to the FIFO
+    uint32_t fresh_n = 0;  // fresh ids of the query (= fifo_tail unless the screen dropped some); the log holds them
+    auto fresh_tail = [&]() { return kScreen ? fresh_n : fifo_tail; };
 
     // ---- best-first loop (SearchImpl) ----
     for (;;) {
@@ -486,12 +606,12 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
       }
       // a step inserts at most nslots ids: move to the bitmap before the hash set could pass 3/4 full.  Every id the
       // query has visited is a seed or in the log (fifo_tail <= vset_max < vlog_cap).  Block-uniform.
-      if (hashed && L + fifo_tail + static_cast<uint32_t>(nslots) > static_cast<uint32_t>(a.vset_max)) {
+      if (hashed && L + fresh_tail() + static_cast<uint32_t>(nslots) > static_cast<uint32_t>(a.vset_max)) {
         for (int i = tid; i < L; i += kGsThreads) {
           const uint32_t id = static_cast<uint32_t>(a.init_ids[i]);
           atomicOr(&visited[id >> 5], 1u << (id & 31));
         }
-        for (uint32_t i = tid; i < fifo_tail; i += kGsThreads) {
+        for (uint32_t i = tid; i < fresh_tail(); i += kGsThreads) {
           const uint32_t id = static_cast<uint32_t>(vlog[i]);
           atomicOr(&visited[id >> 5], 1u << (id & 31));
         }
@@ -564,6 +684,7 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
       }
       GS_T(ta1);
       GS_ACC(6, tb1, ta1);
+      if (kScreen && tid < kMaxW * kEll / 32) s_keep[tid] = 0u;
       __syncthreads();  // (2)
       int total = 0;
 #pragma unroll
@@ -575,12 +696,40 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
           total += s_wcnt[r][w];
         }
         if (fr[r]) {
-          const uint32_t at = fifo_tail + static_cast<uint32_t>(mine + __popc(bal[r] & lane_lt));
-          fifo[at & fmask] = nb[r];
-          if (at < static_cast<uint32_t>(a.vlog_cap)) vlog[at] = nb[r];
+          const uint32_t rank = static_cast<uint32_t>(mine + __popc(bal[r] & lane_lt));
+          fifo[(fifo_tail + rank) & fmask] = nb[r];
+          if (fresh_tail() + rank < static_cast<uint32_t>(a.vlog_cap)) vlog[fresh_tail() + rank] = nb[r];
         }
       }
-      fifo_tail += static_cast<uint32_t>(total);
+      if (kScreen) fresh_n += static_cast<uint32_t>(total);
+      // -- A2: screen the fresh ids on their sketches once the queue holds L entries (block-uniform) --
+      const unsigned long long sbound = kScreen ? qa[L - 1] & kKeyMask : kKeyInf;
+      if (kScreen && total > 0 && sbound != kKeyInf) {
+        __syncthreads();  // (3) the fresh ids are in the FIFO, s_keep is clear
+        screen_fresh(a, fifo, fmask, fifo_tail, total, psk, sbound, tid, s_keep);
+        int mine[kMaxW * kEll / kGsThreads];
+#pragma unroll
+        for (int r = 0; r < kMaxW * kEll / kGsThreads; ++r) {
+          const int i = r * kGsThreads + tid;
+          mine[r] = i < total ? fifo[(fifo_tail + static_cast<uint32_t>(i)) & fmask] : -1;
+        }
+        __syncthreads();  // (4) every keep bit is set and every id read: compact the survivors in order
+        int kept = 0;
+        for (int w = 0; w < (total + 31) >> 5; ++w) kept += __popc(s_keep[w]);
+#pragma unroll
+        for (int r = 0; r < kMaxW * kEll / kGsThreads; ++r) {
+          const int i = r * kGsThreads + tid;
+          if (i < total && ((s_keep[i >> 5] >> (i & 31)) & 1u)) {
+            int rank = __popc(s_keep[i >> 5] & ((1u << (i & 31)) - 1u));
+            for (int w = 0; w < (i >> 5); ++w) rank += __popc(s_keep[w]);
+            fifo[(fifo_tail + static_cast<uint32_t>(rank)) & fmask] = mine[r];
+          }
+        }
+        if (tid == 0) st_nscr += static_cast<unsigned long long>(total - kept);
+        fifo_tail += static_cast<uint32_t>(kept);
+      } else {
+        fifo_tail += static_cast<uint32_t>(total);
+      }
       if (cont_mode) {
         if (tid == 0) {
           s_cont_e[ncont - 1] = e0 + nslots;
@@ -632,11 +781,11 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
     if (tid == 0 && !hashed) ++prof_migrated;
 #endif
     if (hashed) continue;
-    if (fifo_tail <= static_cast<uint32_t>(a.vlog_cap) && 10ll * (fifo_tail + L) < a.visited_words) {
+    if (fresh_tail() <= static_cast<uint32_t>(a.vlog_cap) && 10ll * (fresh_tail() + L) < a.visited_words) {
       // large table: clear only the words this query touched (the seeds and the logged fresh ids) instead of
       // streaming zeros over the whole bitmap (1.25 MB per query at 10M rows)
       for (int i = tid; i < L; i += kGsThreads) visited[static_cast<uint32_t>(a.init_ids[i]) >> 5] = 0u;
-      for (uint32_t i = tid; i < fifo_tail; i += kGsThreads) visited[static_cast<uint32_t>(vlog[i]) >> 5] = 0u;
+      for (uint32_t i = tid; i < fresh_tail(); i += kGsThreads) visited[static_cast<uint32_t>(vlog[i]) >> 5] = 0u;
     } else {
       uint4* v4 = reinterpret_cast<uint4*>(visited);
       const int64_t n4 = a.visited_words >> 2;
@@ -650,6 +799,7 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
     if (warp == 0) atomicAdd(&a.stats[24], static_cast<unsigned long long>(clock64() - t_kernel0));
   }
   for (int i = 0; i < 5; ++i) if (prefix_cnt[i]) atomicAdd(&a.stats[25 + i], prefix_cnt[i]);
+  for (int i = 0; i < 2; ++i) if (prefix_cnt[5 + i]) atomicAdd(&a.stats[32 + i], prefix_cnt[5 + i]);
   if (prof_vtest) atomicAdd(&a.stats[5], prof_vtest);
   if (prof_migrated) atomicAdd(&a.stats[30], prof_migrated);
   if (vacc) atomicAdd(&a.stats[31], vacc);
@@ -657,6 +807,7 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
   if (st_ndist) atomicAdd(&a.stats[0], st_ndist);
   if (st_nexp) atomicAdd(&a.stats[1], st_nexp);
   if (st_nedge) atomicAdd(&a.stats[2], st_nedge);
+  if (st_nscr) atomicAdd(a.n_screened, st_nscr);
 }
 
 __global__ void csr_to_ell_kernel(const int64_t* __restrict__ offsets, const int32_t* __restrict__ nbrs, int64_t n,
@@ -758,16 +909,17 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   int R = ring_slots_for(ix, slot_bytes);
   // FIFO: a backlog below R entries + the ids one A step appends (W adjacency rows or one 128-id continuation chunk)
   const int fc = next_pow2(std::max(width * kEll, kGsThreads) + kMaxR);
+  const bool screen = screen_on(ix);  // the query sketch takes shared memory only when the screen runs
   auto smem_for = [&](int r) {
     return static_cast<size_t>(r) * slot_bytes + static_cast<size_t>(Lp) * 8 + 2 * kPC * 8 + kMaxR * 8 +
-           static_cast<size_t>(dimp) * 4 + kPC * 4 + static_cast<size_t>(fc) * 4 + kMaxR * 4 + static_cast<size_t>((Lp + 31) / 32) * 4;
+           static_cast<size_t>(dimp) * 4 + (screen ? (kSketch + 4) * 4 : 0) + kPC * 4 + static_cast<size_t>(fc) * 4 + kMaxR * 4 + static_cast<size_t>((Lp + 31) / 32) * 4;
   };
   while (R > 2 && smem_for(R) > 200 * 1024) --R;
   if (smem_for(R) > 226 * 1024) return fail(EPS_ERR_UNSUPPORTED, "queue + query + row ring do not fit in shared memory");
-  EPS_CUDA(cudaFuncSetAttribute(graph_search_kernel<7>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_for(R))));
-  EPS_CUDA(cudaFuncSetAttribute(graph_search_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_for(R))));
+  for (auto k : {graph_search_kernel<7, false>, graph_search_kernel<4, false>, graph_search_kernel<7, true>, graph_search_kernel<4, true>})
+    EPS_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_for(R))));
   auto resident = [&](int r, int* out) {
-    EPS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(out, graph_search_kernel<7>, kGsThreads, smem_for(r)));
+    EPS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(out, graph_search_kernel<7, false>, kGsThreads, smem_for(r)));
     if (*out < 1) *out = 1;
     if (ix->graph_ctas_per_sm > 0) *out = std::min(*out, ix->graph_ctas_per_sm);
     return EPS_OK;
@@ -796,9 +948,9 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
     slots = static_cast<int>(std::min<int64_t>(nq, static_cast<int64_t>(per_sm) * ix->num_sms));
   VisitedSets vis;
   EPS_TRY(prepare_visited(ix, slots, L, &vis));
-  EPS_TRY(ix->s_misc.reserve(256));  // [0..3] counters, [+32 B] work counter, [5] [30..31] developer hash-set counts,
-                                     // [8..24] developer phase timers, [25..29] developer prefix counts
-  EPS_CUDA(cudaMemsetAsync(ix->s_misc.p, 0, 256, ix->stream));
+  EPS_TRY(ix->s_misc.reserve(512));  // [0..3] counters, [+32 B] work counter, [5] [30..31] developer hash-set counts,
+                                     // [8..24] developer phase timers, [25..29] [32..33] developer prefix / sketch counts
+  EPS_CUDA(cudaMemsetAsync(ix->s_misc.p, 0, 512, ix->stream));
   uint64_t launches = 1;
   EPS_TRY(ensure_ell(ix, &launches));
   if (ix->seed_rows_L != L) {  // contiguous copy of the query-independent seed rows
@@ -826,16 +978,48 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   a.vec4 = ix->vec4 ? 1 : 0; a.L = static_cast<int>(L); a.Lp = Lp; a.nq = static_cast<int>(nq);
   a.W = width; a.R = R; a.slot_bytes = slot_bytes; a.fc = fc;
   a.qtimes = nullptr;
+  a.sk = nullptr; a.qsk = nullptr; a.n_sk = 0; a.sk_g = 0.f; a.sk_scale = 0.f; a.n_screened = nullptr;
+  if (screen) {
+    if (!ix->d_screened) {
+      EPS_CUDA(cudaMalloc(&ix->d_screened, 8));
+      EPS_CUDA(cudaMemsetAsync(ix->d_screened, 0, 8, ix->stream));
+    }
+    EPS_TRY(ix->s_qsk.reserve(static_cast<size_t>(nq) * (kSketch + 1) * 4));
+    float* qsk = ix->s_qsk.as<float>();
+    EPS_TRY(sketch_rows(ix, d_queries, nq, qsk, qsk + nq * kSketch));
+    ++launches;
+    a.sk = ix->d_sk; a.qsk = qsk; a.n_sk = ix->n_indexed; a.sk_g = ix->sk_g; a.sk_scale = ix->sk_scale;
+    a.n_screened = ix->d_screened;
+  }
+
 #ifdef EPS_GS_PROFILE
   EPS_TRY(ix->s_tail.reserve(static_cast<size_t>(nq) * 32));  // borrowed scratch (the hybrid tail buffer is filled after the search)
   a.qtimes = ix->s_tail.as<unsigned long long>();
   ix->prof_nq = nq;
+  a.prof_basis = nullptr;
+  a.prof_m = 64;
+  if (ix->metric == EPS_METRIC_L2 && staged && dim >= a.prof_m) {
+    if (ix->prof_basis_rows != ix->n_indexed) {
+      std::vector<float> basis, mean;
+      double share = 0;
+      EPS_TRY(principal_subspace(ix, a.prof_m, &basis, &mean, &share));
+      EPS_TRY(ix->s_prof_basis.reserve(basis.size() * 4));
+      EPS_CUDA(cudaMemcpyAsync(ix->s_prof_basis.p, basis.data(), basis.size() * 4, cudaMemcpyHostToDevice, ix->stream));
+      EPS_CUDA(cudaStreamSynchronize(ix->stream));
+      ix->prof_basis_rows = ix->n_indexed;
+      fprintf(stderr, "[gs-profile] principal subspace of %lld rows: the top %d components carry %.4f of the variance\n",
+              static_cast<long long>(ix->n_indexed), a.prof_m, share);
+    }
+    a.prof_basis = ix->s_prof_basis.as<float>();
+  }
 #endif
   // at most 4 resident CTAs per SM (what the auto rule picks for batches above one wave at 7 per SM, e.g. 1024 queries
   // at L = 768): the register file has room for 128 registers per thread, so the instance that hardly spills runs;
   // smaller batches keep 7 resident queries per SM
-  if (per_sm <= 4) graph_search_kernel<4><<<slots, kGsThreads, smem, ix->stream>>>(a);
-  else graph_search_kernel<7><<<slots, kGsThreads, smem, ix->stream>>>(a);
+  if (per_sm <= 4 && screen) graph_search_kernel<4, true><<<slots, kGsThreads, smem, ix->stream>>>(a);
+  else if (per_sm <= 4) graph_search_kernel<4, false><<<slots, kGsThreads, smem, ix->stream>>>(a);
+  else if (screen) graph_search_kernel<7, true><<<slots, kGsThreads, smem, ix->stream>>>(a);
+  else graph_search_kernel<7, false><<<slots, kGsThreads, smem, ix->stream>>>(a);
   EPS_CUDA(cudaGetLastError());
   if (stats) {
     stats->n_seed += static_cast<uint64_t>(nq) * static_cast<uint64_t>(L);
@@ -888,8 +1072,8 @@ int read_graph_counters(Index* ix, eps_stats* stats) {
   stats->n_expand += h[1];
   stats->n_edges += h[2];
 #ifdef EPS_GS_PROFILE
-  unsigned long long pr[32];
-  EPS_CUDA(cudaMemcpy(pr, ix->s_misc.p, 256, cudaMemcpyDeviceToHost));
+  unsigned long long pr[64];
+  EPS_CUDA(cudaMemcpy(pr, ix->s_misc.p, 512, cudaMemcpyDeviceToHost));
   const char* names[8] = {"barrierX", "merge", "row_wait", "team_phase", "pick", "barrier1", "adj+visited", "barrier2+fifo"};
   const double tot = static_cast<double>(pr[24]) + 1.0;
   fprintf(stderr, "[gs-profile] kernel cycles summed over CTAs %.3e;", tot);
@@ -909,6 +1093,9 @@ int read_graph_counters(Index* ix, eps_stats* stats) {
       fprintf(stderr, " %d/4 %.4f (%.4f)", j, p, s + (1.0 - p) * (1.0 - s));
     }
     fprintf(stderr, "\n");
+    // fetching a sketch of b bytes for every evaluated row and the row only where the sketch cannot reject it
+    fprintf(stderr, "[gs-profile] share of those rows whose principal-subspace bound fails the bound: 32 floats %.4f, 64 floats %.4f\n",
+            static_cast<double>(pr[32]) / static_cast<double>(pr[25]), static_cast<double>(pr[33]) / static_cast<double>(pr[25]));
   }
   if (ix->prof_nq > 0 && ix->s_tail.p) {
     std::vector<unsigned long long> t(static_cast<size_t>(ix->prof_nq) * 4);

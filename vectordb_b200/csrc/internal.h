@@ -108,6 +108,21 @@ struct Index {
   size_t vset_clean_cap = 0;
   bool graph_counters_pending = false;
   int64_t prof_nq = 0;           // developer build (EPS_GS_PROFILE): queries of the last profiled launch
+  DevBuf s_prof_basis;           // developer build: principal subspace of the first prof_basis_rows rows (sketch.cu)
+  int64_t prof_basis_rows = 0;
+
+  // principal-subspace sketch of the indexed rows (sketch.cu), computed when a graph is installed; a view shares its
+  // base's.  Dropped with the graph or the rows under it.
+  int graph_screen = EPS_GRAPH_SCREEN_AUTO;
+  int sk_m = 0;                  // floats per row sketch: kSketch, or 0 while there is no basis
+  double sk_share = -1.0;        // share of the sampled variance the basis carries; -1 = no basis
+  float sk_g = 0.f;              // 1 - gamma_{m+2}, rounded down
+  float sk_scale = 0.f;          // (1 - 2 (dim + 2) 2^-24) / (1 + eps), rounded down
+  double sk_eps = 0.0;           // sigma_max(P~)^2 <= 1 + sk_eps
+  float* d_sk_basis = nullptr;   // [dim x sk_m] fp32 basis P~ (transposed), then [dim] mean
+  float* d_sk = nullptr;         // [n_indexed x sk_m] row sketches, then [n_indexed] their error bounds (null: screen off)
+  DevBuf s_qsk;                  // [nq x sk_m] query sketches, then [nq] their error bounds
+  unsigned long long* d_screened = nullptr;  // device count of the fresh neighbours the screen dropped on this handle
   void* h_out = nullptr;         // pinned host mirror of the packed result block (eps_search_batch)
   size_t h_out_cap = 0;
 };
@@ -203,6 +218,22 @@ struct VisitedSets {
   int vlog_cap;
 };
 int prepare_visited(Index* ix, int slots, int64_t L, VisitedSets* v);
+
+// ---- sketch.cu -----------------------------------------------------------------------------
+constexpr int kSketch = 32;       // floats per row sketch of the graph screen
+// Top-m principal subspace of the first n_indexed rows: basis [m x dim] row-major with orthonormal rows (the first k
+// rows span the top-k subspace), the sample mean [dim], and the share of the sample's variance the m rows carry.
+int principal_subspace(Index* ix, int m, std::vector<float>* basis, std::vector<float>* mean, double* share);
+// The graph search screens fresh neighbours with the sketch when the metric is L2 and the mode is on, or auto with the
+// basis carrying at least kScreenShare of the variance.
+constexpr double kScreenShare = 0.9;
+// Basis (+ row sketches when the screen will run) of the installed graph's rows, at graph install and mode changes.
+// Never fails: a sketch that cannot be set up leaves the screen off.  Row sketches are freed when the screen is off.
+void ensure_sketch(Index* ix);
+void free_sketch(Index* ix);
+bool screen_on(const Index* ix);
+// sketches and error bounds of n rows at d_x (the table's layout) with the index's basis
+int sketch_rows(Index* ix, const float* d_x, int64_t n, float* d_sk, float* d_ex);
 
 // ---- finalize.cu ---------------------------------------------------------------------------
 // Post-filter walk / tail merge of VecSearchExecutor::Search (vec_search_executor.cpp:885-927).

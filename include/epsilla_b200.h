@@ -49,8 +49,17 @@ typedef struct eps_index eps_index;
  * (db/execution/vec_search_executor.cpp:848).
  * Strings: a StringAttr node carries the string-column index in field_offset, a StringConst node the literal's
  * dictionary code in int_value (-1 if the literal is not in the dictionary); string EQ / NE compare codes; the
- * caller lowers `x IN (a, b, ..)` to `x = a OR x = b ..` (integration/epsilla_b200_dropin.cpp does).  LIKE, string
- * concatenation and NEARBY nodes are rejected with EPS_ERR_UNSUPPORTED (regex / geo work, out of scope). */
+ * caller lowers `x IN (a, b, ..)` to `x = a OR x = b ..` (integration/epsilla_b200_dropin.cpp does).
+ * LIKE (node_type 29, query/expr/expr_evaluator.cpp:229-241) takes two children, each a StringAttr or a StringConst
+ * node (anything else: EPS_ERR_UNSUPPORTED); its value type is BOOL.  It matches byte for byte as the reference does:
+ * an empty pattern matches only the empty string, the pattern "%" matches every string, otherwise '%' matches any run
+ * of bytes and '_' one byte, neither across a '\n' or '\r', every other byte is a literal, case-sensitive, and the
+ * pattern must cover the whole string.  The strings behind the codes come from eps_index_append_string_dictionary: a
+ * LIKE literal's code must be a mirrored code, and a column a LIKE reads must hold mirrored codes only; otherwise the
+ * search fails with EPS_ERR_INVALID_ARGUMENT before any launch.  Each call evaluates its LIKE nodes once, on the
+ * device, before the search: per dictionary code when one side is a literal, per row when both are columns.  Strings
+ * and patterns of any length are matched.  String concatenation and NEARBY nodes are rejected with
+ * EPS_ERR_UNSUPPORTED. */
 typedef struct eps_filter_node {
   int64_t node_type;
   int64_t value_type;
@@ -72,7 +81,7 @@ typedef struct eps_stats {
   uint64_t n_queries;
   double kernel_ms;    /* device time of the dominant kernel(s) of this call (CUDA events) */
   double total_ms;     /* device time of the whole call incl. copies (CUDA events) */
-  uint64_t kernel_launches;
+  uint64_t kernel_launches; /* launches of this call's search, the LIKE match pass included */
   uint64_t n_redone;   /* exact scan: queries the coarse-pass guard sent back (fp32 scan or a larger candidate list) */
 } eps_stats;
 
@@ -153,8 +162,22 @@ EPS_API int eps_index_set_attrs(eps_index* ix, const char* attribute_table, int6
 /* String columns (TableSegmentMVP::var_len_attr_table_[column], db/table_segment_mvp.hpp:82) are mirrored as
  * DICTIONARY CODES: the caller keeps one string -> int32 dictionary per table and appends the codes of new rows
  * [first_row, first_row + count) here; filter nodes then compare codes (query/expr/expr_evaluator.cpp:110-125,
- * :176-190: StrEvaluate / string EQ, NE / IN).  column = the field's index in var_len_attr_table_ (< 8). */
+ * :176-190: StrEvaluate / string EQ, NE / IN).  column = the field's index in var_len_attr_table_ (< 8).
+ * Rows may be written again (first_row below the rows already mirrored).  For LIKE the call also records the range of
+ * the column's codes on the host; that range only widens, unless a call rewrites every row from row 0.  So after a
+ * partial rewrite that removes an out-of-range code, a LIKE on the column is still refused until the whole column is
+ * written again. */
 EPS_API int eps_index_set_string_codes(eps_index* ix, int column, int64_t first_row, const int32_t* codes, int64_t count);
+
+/* The strings of dictionary codes [first_code, first_code + count), for LIKE: code first_code + i is
+ * bytes[offsets[i] .. offsets[i+1]) (offsets[0] need not be 0; any byte, NUL included).  Append-only: first_code must
+ * equal the number of codes already mirrored.  A LIKE literal gets a code like any other string (the caller adds it
+ * to its dictionary and appends its bytes), so a row with the same text later gets the same code.  One dictionary per
+ * index; views share it, and appending while the index has live views fails like every other mirror update.  A gap,
+ * a negative count, null buffers or offsets that go backwards: EPS_ERR_INVALID_ARGUMENT; more than 2^31 - 1 codes in
+ * all: EPS_ERR_UNSUPPORTED. */
+EPS_API int eps_index_append_string_dictionary(eps_index* ix, int64_t first_code, int64_t count, const int64_t* offsets,
+                                               const char* bytes);
 
 /* Executor parameters snapshotted at construction (db/table_mvp.cpp:83-87): L_master, L_local
  * (config.hpp MasterQueueSize / LocalQueueSize), prefilter_enabled_.  force_brute != 0 makes every

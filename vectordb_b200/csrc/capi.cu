@@ -80,15 +80,28 @@ int lower_filter(const eps_filter_node* nodes, int64_t n, FilterProg* out) {
       case NT_NOT:
         if (s.left < 0 || s.left >= i) return fail(EPS_ERR_INVALID_ARGUMENT, "filter NOT child must precede the node");
         break;
+      case NT_LIKE: {
+        if (s.left < 0 || s.left >= i || s.right < 0 || s.right >= i)
+          return fail(EPS_ERR_INVALID_ARGUMENT, "filter node children must precede the node");
+        const int64_t lt = nodes[s.left].node_type, rt = nodes[s.right].node_type;
+        if ((lt != NT_StringAttr && lt != NT_StringConst) || (rt != NT_StringAttr && rt != NT_StringConst))
+          return fail(EPS_ERR_UNSUPPORTED, "LIKE operands must be string columns or literals (concatenation is out of scope)");
+        break;
+      }
       default:
         return fail(EPS_ERR_UNSUPPORTED,
-                    "filter node type " + std::to_string(t) + " (LIKE / IN not lowered to OR / geo / aggregation) is out of scope");
+                    "filter node type " + std::to_string(t) + " (IN not lowered to OR / geo / aggregation) is out of scope");
     }
     d.type = static_cast<int16_t>(t);
     d.vtype = static_cast<int16_t>(s.value_type);
     d.left = static_cast<int16_t>(s.left < 0 ? 0 : s.left);
     d.right = static_cast<int16_t>(s.right < 0 ? 0 : s.right);
     d.field_offset = static_cast<int32_t>(s.field_offset);
+    if (t == NT_LIKE) {  // which bit prog_run reads (filter.cuh)
+      const bool lc = nodes[s.left].node_type == NT_StringConst, rc = nodes[s.right].node_type == NT_StringConst;
+      d.vtype = VT_BOOL;
+      d.field_offset = lc && rc ? kLikeConst : (!lc && !rc ? kLikeByRow : (lc ? d.right : d.left));
+    }
   }
   out->n = static_cast<int>(n);
   const FNode& r = out->nodes[n - 1];
@@ -170,6 +183,7 @@ int bind_program_columns(Index* ix, FilterProg* prog) {
       prog->str_col[nd.field_offset] = sc.d_codes;
       continue;
     }
+    if (nd.type == NT_LIKE) continue;  // its field_offset selects a bit (check_like below)
     if (width == 0 || nd.field_offset < 0) continue;  // constants, operators, the @distance pseudo-field
     if (!ix->d_attrs) return fail(EPS_ERR_INVALID_ARGUMENT, "expression reads attributes but eps_index_set_attrs was not called");
     if (static_cast<int64_t>(nd.field_offset) + width > ix->attr_stride)
@@ -177,7 +191,7 @@ int bind_program_columns(Index* ix, FilterProg* prog) {
     if (ix->attr_rows < ix->n_rows)
       return fail(EPS_ERR_INVALID_ARGUMENT, "attribute mirror has fewer rows than the vector mirror (call eps_index_set_attrs)");
   }
-  return EPS_OK;
+  return check_like(ix, *prog);
 }
 
 // What the graph branch of Search needs from a query batch: the graph search of its queries over [0, n_indexed), and
@@ -252,8 +266,10 @@ static int search_device(Index* ix, const float* d_queries, int64_t nq, int64_t 
   FilterProg h_prog;
   EPS_TRY(lower_filter(filter, n_filter, &h_prog));
   const FilterProg* d_prog = nullptr;
+  uint64_t like_launches = 0;
   if (h_prog.n > 0) {
     EPS_TRY(bind_program_columns(ix, &h_prog));
+    EPS_TRY(bind_like(ix, &h_prog, 1, &like_launches));
     EPS_TRY(ix->s_filter.reserve(sizeof(FilterProg)));
     EPS_CUDA(cudaMemcpyAsync(ix->s_filter.p, &h_prog, sizeof(FilterProg), cudaMemcpyHostToDevice, ix->stream));
     // h_prog lives on this stack frame until the sync at the end of the caller's timing region; the copy
@@ -265,6 +281,7 @@ static int search_device(Index* ix, const float* d_queries, int64_t nq, int64_t 
   const bool brute = ix->prefilter || ix->force_brute || n_indexed < 512;  // BruteforceThreshold (hpp:28)
   eps_stats local;
   std::memset(&local, 0, sizeof(local));
+  local.kernel_launches = like_launches;  // the LIKE pass
   if (stats) EPS_CUDA(cudaEventRecord(ix->ev[1], ix->stream));
   if (brute) {
     // :857 prefilter: min(size, limit); :864 brute: min(size, limit, L_local).  Only that many entries are ever
@@ -303,8 +320,10 @@ static int search_sparse_device(Index* ix, const SparseQueries& q, int64_t nq, i
   FilterProg h_prog;
   EPS_TRY(lower_filter(filter, n_filter, &h_prog));
   const FilterProg* d_prog = nullptr;
+  uint64_t like_launches = 0;
   if (h_prog.n > 0) {
     EPS_TRY(bind_program_columns(ix, &h_prog));
+    EPS_TRY(bind_like(ix, &h_prog, 1, &like_launches));
     EPS_TRY(ix->s_filter.reserve(sizeof(FilterProg)));
     EPS_CUDA(cudaMemcpyAsync(ix->s_filter.p, &h_prog, sizeof(FilterProg), cudaMemcpyHostToDevice, ix->stream));
     d_prog = ix->s_filter.as<FilterProg>();
@@ -316,6 +335,7 @@ static int search_sparse_device(Index* ix, const SparseQueries& q, int64_t nq, i
   dist.metric = ix->metric;
   eps_stats local;
   std::memset(&local, 0, sizeof(local));
+  local.kernel_launches = like_launches;  // the LIKE pass
   if (stats) EPS_CUDA(cudaEventRecord(ix->ev[1], ix->stream));
   const bool graph = ix->sparse_search == EPS_SPARSE_SEARCH_GRAPH && !ix->prefilter && !ix->force_brute &&
                      ix->n_indexed >= 512;  // BruteforceThreshold (hpp:28)
@@ -442,6 +462,7 @@ void eps_index_destroy(eps_index* h) {
       v->d_attrs = nullptr; v->attr_rows = 0;
       v->d_sp_ptr = nullptr; v->d_sp_elems = nullptr; v->d_sp_norm2 = nullptr; v->sp_nnz = 0;
       for (auto& sc : v->str_cols) sc = eps::StrCol();
+      v->dict = eps::StrDict();
     }
     ix->views.clear();
     eps::free_graph(ix);
@@ -449,6 +470,7 @@ void eps_index_destroy(eps_index* h) {
     if (ix->d_deleted) cudaFree(ix->d_deleted);
     if (ix->d_attrs) cudaFree(ix->d_attrs);
     for (auto& sc : ix->str_cols) if (sc.d_codes) cudaFree(sc.d_codes);
+    eps::free_dict(&ix->dict);
     if (ix->d_sp_ptr) cudaFree(ix->d_sp_ptr);
     if (ix->d_sp_elems) cudaFree(ix->d_sp_elems);
     if (ix->d_sp_norm2) cudaFree(ix->d_sp_norm2);
@@ -456,7 +478,7 @@ void eps_index_destroy(eps_index* h) {
   eps::DevBuf* bufs[] = {&ix->s_queries, &ix->s_dist, &ix->s_topk, &ix->s_topk2, &ix->s_pass, &ix->s_filter,
                          &ix->s_vset, &ix->s_visited, &ix->s_vlog, &ix->s_queue, &ix->s_tail, &ix->s_out_ids, &ix->s_out_dists,
                          &ix->s_out_counts, &ix->s_stats, &ix->s_misc, &ix->s_seed_rows, &ix->s_seed_dist, &ix->s_xnorm, &ix->s_qnorm, &ix->s_coarse, &ix->s_thr, &ix->s_cand, &ix->s_cand_cnt, &ix->s_bf16, &ix->s_qbf16, &ix->s_flags, &ix->s_sparse_q, &ix->s_xnorm_max,
-                         &ix->s_qsk};
+                         &ix->s_qsk, &ix->s_like, &ix->s_like_jobs};
   for (auto* b : bufs) b->release();
   if (ix->h_out) cudaFreeHost(ix->h_out);
   if (ix->d_screened) cudaFree(ix->d_screened);
@@ -491,6 +513,7 @@ int eps_index_create_view(eps_index* base_h, eps_index** out) {
   ix->d_attrs = base->d_attrs; ix->attr_stride = base->attr_stride; ix->attr_rows = base->attr_rows;
   ix->attr_cap_rows = base->attr_cap_rows;
   for (int i = 0; i < eps::kMaxStringCols; ++i) ix->str_cols[i] = base->str_cols[i];
+  ix->dict = base->dict;
   ix->L_master = base->L_master; ix->L_local = base->L_local; ix->prefilter = base->prefilter; ix->force_brute = base->force_brute;
   ix->search_width = base->search_width; ix->sparse_search = base->sparse_search; ix->graph_ring_slots = base->graph_ring_slots;
   ix->graph_ctas_per_sm = base->graph_ctas_per_sm; ix->num_sms = base->num_sms;
@@ -736,8 +759,23 @@ int eps_index_set_string_codes(eps_index* h, int column, int64_t first_row, cons
     EPS_CUDA(cudaMemcpyAsync(sc.d_codes + first_row, codes, static_cast<size_t>(count) * 4, cudaMemcpyHostToDevice, ix->stream));
     EPS_CUDA(cudaStreamSynchronize(ix->stream));
   }
+  // code range of the mirror, for LIKE (check_like): a rewrite of every row starts afresh, otherwise it only widens
+  if (first_row == 0 && need >= sc.rows) { sc.any_negative = false; sc.max_code = -1; }
+  for (int64_t i = 0; i < count; ++i) {
+    sc.any_negative |= codes[i] < 0;
+    sc.max_code = std::max(sc.max_code, codes[i]);
+  }
   sc.rows = std::max(sc.rows, need);
   return EPS_OK;
+}
+
+int eps_index_append_string_dictionary(eps_index* h, int64_t first_code, int64_t count, const int64_t* offsets,
+                                       const char* bytes) {
+  Index* ix = reinterpret_cast<Index*>(h);
+  if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");
+  EPS_TRY(eps::check_device(ix->device));
+  EPS_TRY(check_mutable(ix));
+  return eps::dict_append(ix, first_code, count, offsets, bytes);
 }
 
 int eps_index_config(eps_index* h, int64_t L_master, int64_t L_local, int prefilter, int force_brute) {

@@ -135,6 +135,7 @@ extern "C" int eps_facet_batch(eps_index* h, const int64_t* ids, const double* d
     const int64_t q = i / limit;
     if (i % limit < counts[q] && (ids[i] < 0 || ids[i] >= ix->n_rows)) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "result id outside the mirrored rows");
   }
+  EPS_TRY(eps::bind_like(ix, progs.data(), static_cast<int>(progs.size()), nullptr));  // the programs' bitmaps share ix->s_like
   const size_t nl = static_cast<size_t>(nq) * limit;
   eps::DevBuf d_ids, d_dists, d_counts, d_progs, d_keys, d_vals, d_okeys, d_ovals, d_groups;
   EPS_TRY(d_ids.reserve(nl * 8));

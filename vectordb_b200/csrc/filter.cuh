@@ -10,7 +10,13 @@
 //  * strings (SURVEY.md §8f-4): a string column is mirrored as DICTIONARY CODES (int32 per row, one dictionary per
 //    table so codes compare across columns); StringAttr reads the row's code, StringConst carries the literal's
 //    code (-1: literal absent from the dictionary, equal to no row), and string EQ / NE (:186-190) compare codes.
-//    IN (:176-185) is lowered by the caller to an OR of EQs; LIKE and string concatenation stay out of scope.
+//    IN (:176-185) is lowered by the caller to an OR of EQs; string concatenation stays out of scope.
+//  * LIKE (:229-241): the strings behind the codes are mirrored as a dictionary (StrDict), and the match kernel
+//    (like.cu) evaluates every LIKE node of a call once, before the search kernels, into a bitmap: one bit per
+//    dictionary code when one side is a constant, one bit per row when both sides are columns, one bit when both are
+//    constants.  prog_run only reads the bit: FNode.pad is the node's word offset in FilterProg.like_bits and
+//    FNode.field_offset says which bit (kLikeByRow: bit `row`; kLikeConst: bit 0; otherwise the index of the child
+//    whose value is the code to read).
 // The parser emits children before parents, so one forward pass over the node array evaluates the
 // tree without recursion.
 #pragma once
@@ -20,6 +26,8 @@ namespace eps {
 
 constexpr int kMaxFilterNodes = 64;
 constexpr int kMaxStringCols = 8;
+constexpr int kLikeByRow = -1;  // FNode.field_offset of a LIKE whose two sides are columns
+constexpr int kLikeConst = -2;  // ... whose two sides are constants
 
 enum NodeType : int {  // query/expr/expr_types.hpp:11-48
   NT_Invalid, NT_IntConst, NT_StringConst, NT_DoubleConst, NT_BoolConst, NT_Int1Attr, NT_Int2Attr, NT_Int4Attr,
@@ -35,7 +43,7 @@ struct FNode {
   int16_t vtype;
   int16_t left, right;
   int32_t field_offset;
-  int32_t pad;
+  int32_t pad;    // LIKE: word offset of the node's bits in FilterProg.like_bits
   double value;  // IntConst (as double, like NumEvaluate's static_cast), DoubleConst, BoolConst(0/1)
 };
 
@@ -45,6 +53,7 @@ struct FilterProg {
   int root_uses_dist; // root is a numeric comparison (the only place the real distance is visible)
   int pad;
   const int32_t* str_col[kMaxStringCols];  // device columns of dictionary codes (filled when the program is lowered)
+  const uint32_t* like_bits;               // LIKE bitmaps of this program (filled by bind_like)
   FNode nodes[kMaxFilterNodes];
 };
 
@@ -99,6 +108,12 @@ __device__ __forceinline__ void prog_run(const FilterProg& p, const char* __rest
       case NT_GTE: b = num[nd.left] >= num[nd.right]; break;
       case NT_LT: b = num[nd.left] < num[nd.right]; break;
       case NT_LTE: b = num[nd.left] <= num[nd.right]; break;
+      case NT_LIKE: {
+        const int64_t bit = nd.field_offset >= 0 ? static_cast<int64_t>(num[nd.field_offset])
+                                                 : (nd.field_offset == kLikeByRow ? row : 0);
+        b = (p.like_bits[nd.pad + (bit >> 5)] >> (bit & 31)) & 1u;
+        break;
+      }
       default: break;
     }
     num[i] = v;

@@ -28,6 +28,17 @@ struct DevBuf {
 struct StrCol {
   int32_t* d_codes = nullptr;
   int64_t rows = 0, cap = 0;
+  bool any_negative = false;  // some mirrored code is < 0 (a LIKE cannot read the column then)
+  int32_t max_code = -1;      // largest mirrored code
+};
+
+// Device mirror of the caller's string dictionary (like.cu): code c is bytes[off[c] .. off[c+1]).  Append-only,
+// grown like StrCol; a view shares its base's.
+struct StrDict {
+  int64_t* d_off = nullptr;  // [n + 1], d_off[0] = 0
+  char* d_bytes = nullptr;
+  int64_t n = 0, cap = 0;               // codes mirrored / room for codes
+  int64_t bytes = 0, byte_cap = 0;
 };
 
 struct Index {
@@ -75,6 +86,7 @@ struct Index {
   int64_t attr_cap_rows = 0;
   const char* attr_src = nullptr;  // host table the mirror was filled from (append detection)
   StrCol str_cols[kMaxStringCols];
+  StrDict dict;
 
   // executor parameters
   int64_t L_master = 500, L_local = 500;
@@ -92,7 +104,7 @@ struct Index {
   // scratch
   DevBuf s_queries, s_dist, s_topk, s_topk2, s_pass, s_filter, s_vset, s_visited, s_vlog, s_queue, s_tail, s_out_ids, s_out_dists,
       s_out_counts, s_stats, s_misc, s_seed_rows, s_seed_dist, s_xnorm, s_qnorm, s_coarse, s_thr, s_cand, s_cand_cnt, s_bf16, s_qbf16, s_flags,
-      s_sparse_q, s_xnorm_max;
+      s_sparse_q, s_xnorm_max, s_like, s_like_jobs;
   int coarse_mode = 1;           // exact-scan coarse pass: 0 = fp32 SIMT only, 1 = wgmma TF32, 2 = wgmma bf16 mirror
   int coarse_guard = 1;          // verify the coarse pass after the re-score and redo unsafe queries (brute_force.cu)
   int coarse_boost = 1;          // multiplier of k' learnt by the guard for this table (1, 4, 16, 64)
@@ -275,6 +287,18 @@ struct ConnRepair {
   // entries become out-neighbours of nav; flatten lists + extra edges to the reference CSR
   void flatten(int64_t nav, std::vector<int64_t>* off, std::vector<int32_t>* nb);
 };
+
+// ---- like.cu -------------------------------------------------------------------------------
+// Append codes [first_code, first_code + count) to the dictionary mirror (eps_index_append_string_dictionary).
+int dict_append(Index* ix, int64_t first_code, int64_t count, const int64_t* offsets, const char* bytes);
+void free_dict(StrDict* d);
+// Validation of the LIKE nodes of a lowered program (constant codes and the columns they read); bind_program_columns
+// calls it, so every failure comes before any launch.
+int check_like(const Index* ix, const FilterProg& prog);
+// One match-kernel launch on ix->stream for every LIKE node of progs[0 .. n): the bits go to ix->s_like, each
+// program's like_bits points at its share and each LIKE node's pad at its words.  No launch without LIKE nodes;
+// *launches (if given) counts the launch.
+int bind_like(Index* ix, FilterProg* progs, int n, uint64_t* launches);
 
 // ---- misc kernels (capi.cu) ----------------------------------------------------------------
 int normalize_rows_device(cudaStream_t s, float* d, int64_t n, int64_t dim);

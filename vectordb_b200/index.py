@@ -115,6 +115,15 @@ class Index:
         c = np.ascontiguousarray(codes, np.int32)
         check(self.L.eps_index_set_string_codes(self.h, int(column), int(first_row), _p(c), c.size))
 
+    def append_string_dictionary(self, first_code, strings):
+        """Append the strings of dictionary codes [first_code, first_code + len(strings)) for LIKE filters
+        (eps_index_append_string_dictionary); str is encoded as UTF-8, bytes are taken as they are."""
+        enc = [s.encode("utf-8") if isinstance(s, str) else bytes(s) for s in strings]
+        off = np.zeros(len(enc) + 1, np.int64)
+        np.cumsum([len(b) for b in enc], out=off[1:])
+        buf = np.frombuffer(b"".join(enc) + b"\0", np.uint8)  # never empty: a zero-length string list still has a buffer
+        check(self.L.eps_index_append_string_dictionary(self.h, int(first_code), len(enc), _p(off), _p(buf)))
+
     def config(self, L_master=500, L_local=None, prefilter=False, force_brute=False):
         L_local = L_master if L_local is None else L_local
         check(self.L.eps_index_config(self.h, int(L_master), int(L_local), int(bool(prefilter)), int(bool(force_brute))))
@@ -220,7 +229,7 @@ class SparseIndex(Index):
     """Device mirror of one sparse-vector field (eps_index_create_sparse): rows are appended as CSR.  Searches are exact
     scans by default; set_search_mode("graph") searches the graph that build() installed where the reference would
     (n_indexed >= 512, no prefilter / force_brute), with the reference's results at IntraQueryThreads = 1.  Config,
-    deleted bits, attributes, string codes, facets, build and get_graph work as on Index."""
+    deleted bits, attributes, string codes and dictionary, facets, build and get_graph work as on Index."""
 
     def __init__(self, metric, dim, capacity=0, device=0):
         self.L = load_library()

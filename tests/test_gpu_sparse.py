@@ -279,7 +279,12 @@ def test_sparse_view_searches_concurrently(vdb):
     with pytest.raises(vdb.EpsError):
         ix.append(qs)   # a base with live views is frozen
     v.close()
+    # a base destroyed before its view leaves an empty index behind, not a dangling one
+    v2 = ix.view()
     ix.close()
+    _, _, c2, _ = v2.search(qs, 10)
+    assert (c2 == 0).all()
+    v2.close()
 
 
 def test_sparse_graph_build(vdb):

@@ -211,14 +211,7 @@ static int prune_pass(Index* ix, int64_t n, const unsigned long long* d_knn, int
 }
 
 int install_csr(Index* ix, int64_t n, const int64_t* off, const int32_t* nb, int64_t e, int64_t nav) {
-  if (ix->d_offsets) { cudaFree(ix->d_offsets); ix->d_offsets = nullptr; }
-  if (ix->d_nbrs) { cudaFree(ix->d_nbrs); ix->d_nbrs = nullptr; }
-  if (ix->d_init_ids) { cudaFree(ix->d_init_ids); ix->d_init_ids = nullptr; }
-  if (ix->d_ell) { cudaFree(ix->d_ell); ix->d_ell = nullptr; }
-  free_sketch(ix);
-  ix->seed_rows_L = 0;
-  ix->init_L = 0;
-  ix->n_indexed = 0;
+  free_graph(ix);
   EPS_CUDA(cudaMalloc(&ix->d_offsets, (static_cast<size_t>(n) + 1) * 8));
   EPS_CUDA(cudaMalloc(&ix->d_nbrs, std::max<size_t>(static_cast<size_t>(e), 1) * 4));
   EPS_CUDA(cudaMemcpyAsync(ix->d_offsets, off, (static_cast<size_t>(n) + 1) * 8, cudaMemcpyHostToDevice, ix->stream));

@@ -35,7 +35,7 @@ void DevBuf::release() {
   cap = 0;
 }
 
-static int check_device(int device) {
+int check_device(int device) {
   int n = 0;
   cudaError_t e = cudaGetDeviceCount(&n);
   if (e != cudaSuccess || n <= 0)
@@ -147,7 +147,7 @@ __global__ void narrow_ids_kernel(const int64_t* __restrict__ in, int64_t n, int
   if (v < 0 || v >= limit) { *bad = 1; out[i] = 0; } else out[i] = static_cast<int32_t>(v);
 }
 
-static void free_graph(Index* ix) {
+void free_graph(Index* ix) {
   if (ix->d_offsets) cudaFree(ix->d_offsets);
   if (ix->d_nbrs) cudaFree(ix->d_nbrs);
   if (ix->d_init_ids) cudaFree(ix->d_init_ids);
@@ -194,73 +194,48 @@ int bind_program_columns(Index* ix, FilterProg* prog) {
   return check_like(ix, *prog);
 }
 
-// What the graph branch of Search needs from a query batch: the graph search of its queries over [0, n_indexed), and
-// the exact top-k of rows [n_indexed, total) that feeds the tail merge.
-struct GraphQueries {
-  virtual ~GraphQueries() = default;
-  virtual int search(Index* ix, int64_t L, unsigned long long* d_queue, eps_stats* st) const = 0;
-  virtual int tail(Index* ix, int64_t k, const FilterProg* d_prog, const FilterProg* h_prog, unsigned long long* d_tail,
-                   eps_stats* st) const = 0;
+// A search call's queries, dense or sparse: their graph search over [0, n_indexed) and the exact top-k of rows
+// [row_start, row_end).
+struct QueryBatch {
+  virtual ~QueryBatch() = default;
+  virtual int graph(Index* ix, int64_t L, unsigned long long* d_queue, eps_stats* st) const = 0;
+  virtual int scan(Index* ix, int64_t row_start, int64_t row_end, int64_t k, const FilterProg* d_prog,
+                   const FilterProg* h_prog, bool prefilter, unsigned long long* d_topk, eps_stats* st) const = 0;
 };
 
-struct DenseGraphQueries : GraphQueries {
+struct DenseBatch : QueryBatch {
   const float* d_queries;
   int64_t nq;
-  DenseGraphQueries(const float* q, int64_t n) : d_queries(q), nq(n) {}
-  int search(Index* ix, int64_t L, unsigned long long* d_queue, eps_stats* st) const override {
+  DenseBatch(const float* q, int64_t n) : d_queries(q), nq(n) {}
+  int graph(Index* ix, int64_t L, unsigned long long* d_queue, eps_stats* st) const override {
     return graph_search(ix, d_queries, nq, L, d_queue, st);
   }
-  int tail(Index* ix, int64_t k, const FilterProg* d_prog, const FilterProg* h_prog, unsigned long long* d_tail,
-           eps_stats* st) const override {
-    return brute_force_topk(ix, d_queries, nq, ix->n_indexed, ix->n_rows, k, d_prog, h_prog, false, d_tail, st);
+  int scan(Index* ix, int64_t row_start, int64_t row_end, int64_t k, const FilterProg* d_prog, const FilterProg* h_prog,
+           bool prefilter, unsigned long long* d_topk, eps_stats* st) const override {
+    return brute_force_topk(ix, d_queries, nq, row_start, row_end, k, d_prog, h_prog, prefilter, d_topk, st);
   }
 };
 
-struct SparseGraphQueries : GraphQueries {
+struct SparseBatch : QueryBatch {
   SparseDist dist;
-  explicit SparseGraphQueries(const SparseDist& d) : dist(d) {}
-  int search(Index* ix, int64_t L, unsigned long long* d_queue, eps_stats* st) const override {
+  SparseBatch(const SparseQueries& q, int64_t nq, int metric) {
+    dist.q = q;
+    dist.nq = nq;
+    dist.metric = metric;
+  }
+  int graph(Index* ix, int64_t L, unsigned long long* d_queue, eps_stats* st) const override {
     return sparse_graph_search(ix, dist.q, dist.nq, L, d_queue, st);
   }
-  int tail(Index* ix, int64_t k, const FilterProg* d_prog, const FilterProg* h_prog, unsigned long long* d_tail,
-           eps_stats* st) const override {
-    return scan_topk(ix, dist, dist.nq, ix->n_indexed, ix->n_rows, k, d_prog, h_prog, false, -1, d_tail, st);
+  int scan(Index* ix, int64_t row_start, int64_t row_end, int64_t k, const FilterProg* d_prog, const FilterProg* h_prog,
+           bool prefilter, unsigned long long* d_topk, eps_stats* st) const override {
+    return scan_topk(ix, dist, dist.nq, row_start, row_end, k, d_prog, h_prog, prefilter, -1, d_topk, st);
   }
 };
 
-// The graph branch of Search (:869-933): graph search, exact scan of the rows appended after the build, merge of the
-// two and post-filter walk.  ev[2] is recorded after the graph search when stats are wanted.
-static int graph_branch(Index* ix, const GraphQueries& gq, int64_t nq, int64_t limit, const FilterProg* d_prog,
-                        const FilterProg* h_prog, int64_t* d_ids, float* d_dists, int64_t* d_counts, eps_stats* stats,
-                        eps_stats* local) {
-  const int64_t total = ix->n_rows;
-  const int64_t n_indexed = ix->n_indexed;
-  const int64_t L = std::min<int64_t>(ix->L_master, n_indexed);  // Q1 clamp
-  // :872 min(n_indexed, limit, L_local); the queue row holds L entries, so the merge window is clamped to it
-  // (the reference ties L_local to L_master through setSearchQueueSize; the C ABI accepts them separately)
-  const int64_t search_limit = std::min<int64_t>(std::min<int64_t>(std::min<int64_t>(n_indexed, limit), ix->L_local), L);
-  EPS_TRY(ix->s_queue.reserve(static_cast<size_t>(nq) * L * 8));
-  EPS_TRY(gq.search(ix, L, ix->s_queue.as<unsigned long long>(), local));
-  ix->graph_counters_pending = true;
-  if (stats) EPS_CUDA(cudaEventRecord(ix->ev[2], ix->stream));
-  const unsigned long long* d_tail = nullptr;
-  int64_t tail_k = 0;
-  if (total > n_indexed) {  // :885-900
-    // only the first search_limit slots can receive tail entries (:894-900)
-    tail_k = std::min<int64_t>(std::min<int64_t>(limit, total - n_indexed), search_limit);
-    if (tail_k > 8192) return fail(EPS_ERR_UNSUPPORTED, "more than 8192 tail results per query are not supported");
-    EPS_TRY(ix->s_tail.reserve(static_cast<size_t>(nq) * tail_k * 8));
-    EPS_TRY(gq.tail(ix, tail_k, d_prog, h_prog, ix->s_tail.as<unsigned long long>(), local));
-    d_tail = ix->s_tail.as<unsigned long long>();
-  }
-  EPS_TRY(finalize_graph(ix, ix->s_queue.as<unsigned long long>(), nq, L, search_limit, L, d_tail, tail_k, limit,
-                         d_prog, h_prog, d_ids, d_dists, d_counts));
-  local->kernel_launches += 1;
-  return EPS_OK;
-}
-
-static int search_device(Index* ix, const float* d_queries, int64_t nq, int64_t limit, const eps_filter_node* filter,
-                         int64_t n_filter, int64_t* d_ids, float* d_dists, int64_t* d_counts, eps_stats* stats) {
+// VecSearchExecutor::Search (:833-935) of nq queries into device ids / dists / counts.  ev[1] -> ev[2] brackets the
+// search kernels when stats are wanted.
+static int run_search(Index* ix, const QueryBatch& qb, int64_t nq, int64_t limit, const eps_filter_node* filter,
+                      int64_t n_filter, int64_t* d_ids, float* d_dists, int64_t* d_counts, eps_stats* stats) {
   if (nq <= 0) return EPS_OK;
   if (limit < 1) return fail(EPS_ERR_INVALID_ARGUMENT, "limit must be >= 1");
   FilterProg h_prog;
@@ -278,27 +253,47 @@ static int search_device(Index* ix, const float* d_queries, int64_t nq, int64_t 
   }
   const int64_t total = ix->n_rows;
   const int64_t n_indexed = ix->n_indexed;
-  const bool brute = ix->prefilter || ix->force_brute || n_indexed < 512;  // BruteforceThreshold (hpp:28)
   eps_stats local;
   std::memset(&local, 0, sizeof(local));
   local.kernel_launches = like_launches;  // the LIKE pass
   if (stats) EPS_CUDA(cudaEventRecord(ix->ev[1], ix->stream));
-  if (brute) {
+  // BruteforceThreshold (hpp:28); a sparse index in EPS_SPARSE_SEARCH_SCAN always scans, whatever graph is installed
+  const bool graph = !ix->prefilter && !ix->force_brute && n_indexed >= 512 &&
+                     (!ix->sparse || ix->sparse_search == EPS_SPARSE_SEARCH_GRAPH);
+  if (graph) {
+    // :869-933: graph search, exact scan of the rows appended after the build, merge of the two and post-filter walk
+    const int64_t L = std::min<int64_t>(ix->L_master, n_indexed);  // Q1 clamp
+    // :872 min(n_indexed, limit, L_local); the queue row holds L entries, so the merge window is clamped to it
+    // (the reference ties L_local to L_master through setSearchQueueSize; the C ABI accepts them separately)
+    const int64_t search_limit = std::min<int64_t>(std::min<int64_t>(std::min<int64_t>(n_indexed, limit), ix->L_local), L);
+    EPS_TRY(ix->s_queue.reserve(static_cast<size_t>(nq) * L * 8));
+    EPS_TRY(qb.graph(ix, L, ix->s_queue.as<unsigned long long>(), &local));
+    ix->graph_counters_pending = true;
+    if (stats) EPS_CUDA(cudaEventRecord(ix->ev[2], ix->stream));
+    const unsigned long long* d_tail = nullptr;
+    int64_t tail_k = 0;
+    if (total > n_indexed) {  // :885-900
+      // only the first search_limit slots can receive tail entries (:894-900)
+      tail_k = std::min<int64_t>(std::min<int64_t>(limit, total - n_indexed), search_limit);
+      if (tail_k > 8192) return fail(EPS_ERR_UNSUPPORTED, "more than 8192 tail results per query are not supported");
+      EPS_TRY(ix->s_tail.reserve(static_cast<size_t>(nq) * tail_k * 8));
+      EPS_TRY(qb.scan(ix, n_indexed, total, tail_k, d_prog, &h_prog, false, ix->s_tail.as<unsigned long long>(), &local));
+      d_tail = ix->s_tail.as<unsigned long long>();
+    }
+    EPS_TRY(finalize_graph(ix, ix->s_queue.as<unsigned long long>(), nq, L, search_limit, L, d_tail, tail_k, limit,
+                           d_prog, &h_prog, d_ids, d_dists, d_counts));
+  } else {
     // :857 prefilter: min(size, limit); :864 brute: min(size, limit, L_local).  Only that many entries are ever
     // emitted, so the exact top-k is taken for the EFFECTIVE k (a large `limit` on a small table is legal).
     const int64_t cap = (ix->prefilter || ix->force_brute) ? limit : std::min<int64_t>(limit, ix->L_local);
     const int64_t k = std::max<int64_t>(1, std::min<int64_t>(cap, total));
     if (k > 8192) return fail(EPS_ERR_UNSUPPORTED, "more than 8192 results per query from the exact scan are not supported");
     EPS_TRY(ix->s_topk.reserve(static_cast<size_t>(nq) * k * 8));
-    EPS_TRY(brute_force_topk(ix, d_queries, nq, 0, total, k, d_prog, &h_prog, ix->prefilter,
-                             ix->s_topk.as<unsigned long long>(), &local));
+    EPS_TRY(qb.scan(ix, 0, total, k, d_prog, &h_prog, ix->prefilter, ix->s_topk.as<unsigned long long>(), &local));
     if (stats) EPS_CUDA(cudaEventRecord(ix->ev[2], ix->stream));
     EPS_TRY(finalize_keys(ix, ix->s_topk.as<unsigned long long>(), nq, k, limit, cap, d_ids, d_dists, d_counts));
-    local.kernel_launches += 1;
-  } else {
-    EPS_TRY(graph_branch(ix, DenseGraphQueries(d_queries, nq), nq, limit, d_prog, &h_prog, d_ids, d_dists, d_counts, stats,
-                         &local));
   }
+  local.kernel_launches += 1;  // finalize_graph / finalize_keys
   if (stats) {
     stats->n_dist += local.n_dist;
     stats->n_seed += local.n_seed;
@@ -311,54 +306,48 @@ static int search_device(Index* ix, const float* d_queries, int64_t nq, int64_t 
   return EPS_OK;
 }
 
-// search_device for a sparse index.  EPS_SPARSE_SEARCH_SCAN: always the exact scan over [0, total) with the brute-force
-// branch's caps (:857 prefilter: limit; :864 brute: min(limit, L_local)), whatever graph is installed.
-// EPS_SPARSE_SEARCH_GRAPH: the reference's branch rule (:855-868), the graph branch where it applies.
-static int search_sparse_device(Index* ix, const SparseQueries& q, int64_t nq, int64_t limit, const eps_filter_node* filter,
-                                int64_t n_filter, int64_t* d_ids, float* d_dists, int64_t* d_counts, eps_stats* stats) {
-  if (nq <= 0) return EPS_OK;
-  FilterProg h_prog;
-  EPS_TRY(lower_filter(filter, n_filter, &h_prog));
-  const FilterProg* d_prog = nullptr;
-  uint64_t like_launches = 0;
-  if (h_prog.n > 0) {
-    EPS_TRY(bind_program_columns(ix, &h_prog));
-    EPS_TRY(bind_like(ix, &h_prog, 1, &like_launches));
-    EPS_TRY(ix->s_filter.reserve(sizeof(FilterProg)));
-    EPS_CUDA(cudaMemcpyAsync(ix->s_filter.p, &h_prog, sizeof(FilterProg), cudaMemcpyHostToDevice, ix->stream));
-    d_prog = ix->s_filter.as<FilterProg>();
+// The end of a call with stats, after the stream is synchronised: the graph search's counters if it ran, the kernel
+// time ev[1] -> ev[2] and the call's time ev[0] -> ev[3].
+static int finish_stats(Index* ix, eps_stats* stats) {
+  if (ix->graph_counters_pending) {
+    EPS_TRY(read_graph_counters(ix, stats));
+    ix->graph_counters_pending = false;
   }
-  const int64_t total = ix->n_rows;
-  SparseDist dist;
-  dist.q = q;
-  dist.nq = nq;
-  dist.metric = ix->metric;
-  eps_stats local;
-  std::memset(&local, 0, sizeof(local));
-  local.kernel_launches = like_launches;  // the LIKE pass
-  if (stats) EPS_CUDA(cudaEventRecord(ix->ev[1], ix->stream));
-  const bool graph = ix->sparse_search == EPS_SPARSE_SEARCH_GRAPH && !ix->prefilter && !ix->force_brute &&
-                     ix->n_indexed >= 512;  // BruteforceThreshold (hpp:28)
-  if (graph) {
-    EPS_TRY(graph_branch(ix, SparseGraphQueries(dist), nq, limit, d_prog, &h_prog, d_ids, d_dists, d_counts, stats, &local));
-  } else {
-    const int64_t cap = (ix->prefilter || ix->force_brute) ? limit : std::min<int64_t>(limit, ix->L_local);
-    const int64_t k = std::max<int64_t>(1, std::min<int64_t>(cap, total));
-    if (k > 8192) return fail(EPS_ERR_UNSUPPORTED, "more than 8192 results per query from the exact scan are not supported");
-    EPS_TRY(ix->s_topk.reserve(static_cast<size_t>(nq) * k * 8));
-    EPS_TRY(scan_topk(ix, dist, nq, 0, total, k, d_prog, &h_prog, ix->prefilter, -1, ix->s_topk.as<unsigned long long>(), &local));
-    if (stats) EPS_CUDA(cudaEventRecord(ix->ev[2], ix->stream));
-    EPS_TRY(finalize_keys(ix, ix->s_topk.as<unsigned long long>(), nq, k, limit, cap, d_ids, d_dists, d_counts));
-    local.kernel_launches += 1;
+  float ms = 0.f;
+  cudaEventElapsedTime(&ms, ix->ev[1], ix->ev[2]);
+  stats->kernel_ms += ms;
+  cudaEventElapsedTime(&ms, ix->ev[0], ix->ev[3]);
+  stats->total_ms += ms;
+  return EPS_OK;
+}
+
+// run_search of queries already on the device, returned to the caller's host arrays: one device block
+// [ids | counts | dists] and one pinned host mirror of it, so a single D2H copy per call.
+static int search_to_host(Index* ix, const QueryBatch& qb, int64_t nq, int64_t limit, const eps_filter_node* filter,
+                          int64_t n_filter, int64_t* out_ids, double* out_dists, int64_t* out_counts, eps_stats* stats) {
+  const size_t n_ids = static_cast<size_t>(nq) * limit;
+  const size_t off_cnt = n_ids * 8, off_dist = off_cnt + static_cast<size_t>(nq) * 8, total = off_dist + n_ids * 4;
+  EPS_TRY(ix->s_out_ids.reserve(total));
+  if (ix->h_out_cap < total) {
+    if (ix->h_out) cudaFreeHost(ix->h_out);
+    ix->h_out = nullptr;
+    ix->h_out_cap = 0;
+    EPS_CUDA(cudaHostAlloc(&ix->h_out, total, cudaHostAllocDefault));
+    ix->h_out_cap = total;
   }
-  if (stats) {
-    stats->n_dist += local.n_dist;
-    stats->n_seed += local.n_seed;
-    stats->n_expand += local.n_expand;
-    stats->n_edges += local.n_edges;
-    stats->n_queries += static_cast<uint64_t>(nq);
-    stats->kernel_launches += local.kernel_launches;
-  }
+  unsigned char* d_blk = ix->s_out_ids.as<unsigned char>();
+  EPS_TRY(run_search(ix, qb, nq, limit, filter, n_filter, reinterpret_cast<int64_t*>(d_blk),
+                     reinterpret_cast<float*>(d_blk + off_dist), reinterpret_cast<int64_t*>(d_blk + off_cnt), stats));
+  EPS_CUDA(cudaMemcpyAsync(ix->h_out, d_blk, total, cudaMemcpyDeviceToHost, ix->stream));
+  if (stats) EPS_CUDA(cudaEventRecord(ix->ev[3], ix->stream));
+  EPS_CUDA(cudaStreamSynchronize(ix->stream));
+  const unsigned char* hb = static_cast<const unsigned char*>(ix->h_out);
+  std::memcpy(out_ids, hb, n_ids * 8);
+  std::memcpy(out_counts, hb + off_cnt, static_cast<size_t>(nq) * 8);
+  const float* hd = reinterpret_cast<const float*>(hb + off_dist);
+  for (size_t i = 0; i < n_ids; ++i) out_dists[i] = static_cast<double>(hd[i]);  // distance_ is vector<double> (hpp:52)
+  if (stats) EPS_TRY(finish_stats(ix, stats));
+  ix->graph_counters_pending = false;
   return EPS_OK;
 }
 
@@ -455,14 +444,9 @@ void eps_index_destroy(eps_index* h) {
     for (Index* v : ix->views) {  // base destroyed before its views: they become empty indexes instead of dangling
       cudaStreamSynchronize(v->stream);
       v->view_of = nullptr; v->detached_view = true;
-      v->d_vectors = nullptr; v->n_rows = 0; v->capacity = 0;
-      v->d_offsets = nullptr; v->d_nbrs = nullptr; v->d_ell = nullptr; v->n_indexed = 0; v->n_edges = 0;
-      eps::free_sketch(v);
-      v->d_deleted = nullptr; v->deleted_bytes = 0; v->any_deleted = false;
-      v->d_attrs = nullptr; v->attr_rows = 0;
-      v->d_sp_ptr = nullptr; v->d_sp_elems = nullptr; v->d_sp_norm2 = nullptr; v->sp_nnz = 0;
-      for (auto& sc : v->str_cols) sc = eps::StrCol();
-      v->dict = eps::StrDict();
+      const int64_t nav = v->nav;  // eps_index_get_graph still reports it
+      static_cast<eps::Table&>(*v) = eps::Table();
+      v->nav = nav;
     }
     ix->views.clear();
     eps::free_graph(ix);
@@ -475,16 +459,11 @@ void eps_index_destroy(eps_index* h) {
     if (ix->d_sp_elems) cudaFree(ix->d_sp_elems);
     if (ix->d_sp_norm2) cudaFree(ix->d_sp_norm2);
   }
-  eps::DevBuf* bufs[] = {&ix->s_queries, &ix->s_dist, &ix->s_topk, &ix->s_topk2, &ix->s_pass, &ix->s_filter,
-                         &ix->s_vset, &ix->s_visited, &ix->s_vlog, &ix->s_queue, &ix->s_tail, &ix->s_out_ids, &ix->s_out_dists,
-                         &ix->s_out_counts, &ix->s_stats, &ix->s_misc, &ix->s_seed_rows, &ix->s_seed_dist, &ix->s_xnorm, &ix->s_qnorm, &ix->s_coarse, &ix->s_thr, &ix->s_cand, &ix->s_cand_cnt, &ix->s_bf16, &ix->s_qbf16, &ix->s_flags, &ix->s_sparse_q, &ix->s_xnorm_max,
-                         &ix->s_qsk, &ix->s_like, &ix->s_like_jobs};
-  for (auto* b : bufs) b->release();
   if (ix->h_out) cudaFreeHost(ix->h_out);
   if (ix->d_screened) cudaFree(ix->d_screened);
   for (auto& ev : ix->ev) if (ev) cudaEventDestroy(ev);
   cudaStreamDestroy(ix->stream);
-  delete ix;
+  delete ix;  // the scratch DevBufs release themselves
 }
 
 // A read-only view of an index: the same device table, graph and segment mirrors, its own stream and scratch.
@@ -501,25 +480,10 @@ int eps_index_create_view(eps_index* base_h, eps_index** out) {
   EPS_CUDA(cudaStreamSynchronize(base->stream));  // uploads, graph install and the adjacency table are complete
   Index* ix = new Index();
   ix->view_of = base;
-  ix->device = base->device; ix->metric = base->metric; ix->dim = base->dim; ix->capacity = base->capacity;
-  ix->host_vectors = nullptr; ix->d_vectors = base->d_vectors; ix->owns_vectors = false; ix->n_rows = base->n_rows;
-  ix->vec4 = base->vec4;
-  ix->sparse = base->sparse; ix->d_sp_ptr = base->d_sp_ptr; ix->d_sp_elems = base->d_sp_elems; ix->d_sp_norm2 = base->d_sp_norm2;
-  ix->sp_nnz = base->sp_nnz; ix->sp_elem_cap = base->sp_elem_cap; ix->sp_row_cap = base->sp_row_cap;
-  ix->n_indexed = base->n_indexed; ix->n_edges = base->n_edges; ix->nav = base->nav;
-  ix->d_offsets = base->d_offsets; ix->d_nbrs = base->d_nbrs; ix->d_ell = base->d_ell;
-  ix->d_deleted = base->d_deleted; ix->deleted_bytes = base->deleted_bytes; ix->deleted_cap = base->deleted_cap;
-  ix->any_deleted = base->any_deleted;
-  ix->d_attrs = base->d_attrs; ix->attr_stride = base->attr_stride; ix->attr_rows = base->attr_rows;
-  ix->attr_cap_rows = base->attr_cap_rows;
-  for (int i = 0; i < eps::kMaxStringCols; ++i) ix->str_cols[i] = base->str_cols[i];
-  ix->dict = base->dict;
-  ix->L_master = base->L_master; ix->L_local = base->L_local; ix->prefilter = base->prefilter; ix->force_brute = base->force_brute;
-  ix->search_width = base->search_width; ix->sparse_search = base->sparse_search; ix->graph_ring_slots = base->graph_ring_slots;
-  ix->graph_ctas_per_sm = base->graph_ctas_per_sm; ix->num_sms = base->num_sms;
-  ix->coarse_mode = base->coarse_mode; ix->coarse_guard = base->coarse_guard; ix->coarse_boost = base->coarse_boost;
-  ix->graph_screen = base->graph_screen; ix->sk_m = base->sk_m; ix->sk_share = base->sk_share; ix->sk_g = base->sk_g;
-  ix->sk_scale = base->sk_scale; ix->sk_eps = base->sk_eps; ix->d_sk_basis = base->d_sk_basis; ix->d_sk = base->d_sk;
+  ix->device = base->device; ix->metric = base->metric; ix->dim = base->dim; ix->sparse = base->sparse;
+  ix->num_sms = base->num_sms;
+  static_cast<eps::Table&>(*ix) = *base;
+  static_cast<eps::Config&>(*ix) = *base;
   cudaError_t e = cudaStreamCreateWithFlags(&ix->stream, cudaStreamNonBlocking);
   if (e != cudaSuccess) { delete ix; return eps::fail(EPS_ERR_CUDA, cudaGetErrorString(e)); }
   for (auto& ev : ix->ev) cudaEventCreate(&ev);
@@ -799,20 +763,12 @@ int eps_search_batch_device(eps_index* h, const float* d_queries, int64_t nq, in
   if (nq <= 0) return EPS_OK;  // nothing launched: no events to read back
   EPS_TRY(eps::check_device(ix->device));
   if (stats) EPS_CUDA(cudaEventRecord(ix->ev[0], ix->stream));
-  EPS_TRY(eps::search_device(ix, d_queries, nq, limit, filter, n_filter, d_out_ids, d_out_dists, d_out_counts, stats));
+  EPS_TRY(eps::run_search(ix, eps::DenseBatch(d_queries, nq), nq, limit, filter, n_filter, d_out_ids, d_out_dists,
+                          d_out_counts, stats));
   if (stats) EPS_CUDA(cudaEventRecord(ix->ev[3], ix->stream));
-  if (!stats) ix->graph_counters_pending = false;
-  if (sync || stats) {
-    EPS_CUDA(cudaStreamSynchronize(ix->stream));
-    if (stats) {
-      if (ix->graph_counters_pending) { EPS_TRY(eps::read_graph_counters(ix, stats)); ix->graph_counters_pending = false; }
-      float ms = 0.f;
-      cudaEventElapsedTime(&ms, ix->ev[1], ix->ev[2]);
-      stats->kernel_ms += ms;
-      cudaEventElapsedTime(&ms, ix->ev[0], ix->ev[3]);
-      stats->total_ms += ms;
-    }
-  }
+  else ix->graph_counters_pending = false;
+  if (sync || stats) EPS_CUDA(cudaStreamSynchronize(ix->stream));
+  if (stats) EPS_TRY(eps::finish_stats(ix, stats));
   return EPS_OK;
 }
 
@@ -825,40 +781,10 @@ int eps_search_batch(eps_index* h, const float* queries, int64_t nq, int64_t lim
   if (limit < 1) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "limit must be >= 1");
   EPS_TRY(eps::check_device(ix->device));
   if (stats) EPS_CUDA(cudaEventRecord(ix->ev[0], ix->stream));
-  // one device block [ids | counts | dists] and one pinned host mirror of it: a single D2H copy per call
-  const size_t n_ids = static_cast<size_t>(nq) * limit;
-  const size_t off_cnt = n_ids * 8, off_dist = off_cnt + static_cast<size_t>(nq) * 8, total = off_dist + n_ids * 4;
   EPS_TRY(ix->s_queries.reserve(static_cast<size_t>(nq) * ix->dim * 4));
-  EPS_TRY(ix->s_out_ids.reserve(total));
-  if (ix->h_out_cap < total) {
-    if (ix->h_out) cudaFreeHost(ix->h_out);
-    ix->h_out = nullptr;
-    ix->h_out_cap = 0;
-    EPS_CUDA(cudaHostAlloc(&ix->h_out, total, cudaHostAllocDefault));
-    ix->h_out_cap = total;
-  }
-  unsigned char* d_blk = ix->s_out_ids.as<unsigned char>();
   EPS_CUDA(cudaMemcpyAsync(ix->s_queries.p, queries, static_cast<size_t>(nq) * ix->dim * 4, cudaMemcpyHostToDevice, ix->stream));
-  EPS_TRY(eps::search_device(ix, ix->s_queries.as<float>(), nq, limit, filter, n_filter, reinterpret_cast<int64_t*>(d_blk),
-                             reinterpret_cast<float*>(d_blk + off_dist), reinterpret_cast<int64_t*>(d_blk + off_cnt), stats));
-  EPS_CUDA(cudaMemcpyAsync(ix->h_out, d_blk, total, cudaMemcpyDeviceToHost, ix->stream));
-  if (stats) EPS_CUDA(cudaEventRecord(ix->ev[3], ix->stream));
-  EPS_CUDA(cudaStreamSynchronize(ix->stream));
-  const unsigned char* hb = static_cast<const unsigned char*>(ix->h_out);
-  std::memcpy(out_ids, hb, n_ids * 8);
-  std::memcpy(out_counts, hb + off_cnt, static_cast<size_t>(nq) * 8);
-  const float* hd = reinterpret_cast<const float*>(hb + off_dist);
-  for (size_t i = 0; i < n_ids; ++i) out_dists[i] = static_cast<double>(hd[i]);  // distance_ is vector<double> (hpp:52)
-  if (stats) {
-    if (ix->graph_counters_pending) { EPS_TRY(eps::read_graph_counters(ix, stats)); ix->graph_counters_pending = false; }
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, ix->ev[1], ix->ev[2]);
-    stats->kernel_ms += ms;
-    cudaEventElapsedTime(&ms, ix->ev[0], ix->ev[3]);
-    stats->total_ms += ms;
-  }
-  ix->graph_counters_pending = false;
-  return EPS_OK;
+  return eps::search_to_host(ix, eps::DenseBatch(ix->s_queries.as<float>(), nq), nq, limit, filter, n_filter, out_ids,
+                             out_dists, out_counts, stats);
 }
 
 int eps_index_append_sparse_rows(eps_index* h, int64_t first_row, int64_t n_rows, const int64_t* offsets,
@@ -887,7 +813,7 @@ int eps_search_sparse_batch(eps_index* h, int64_t nq, const int64_t* q_offsets, 
   std::vector<float> qn;
   EPS_TRY(eps::pack_sparse(nq, q_offsets, q_indices, q_values, 0xffffffffll, 0, &qp, &qe, &qn));
   if (stats) EPS_CUDA(cudaEventRecord(ix->ev[0], ix->stream));
-  // one device block [ptr | norm2 | elems] in, one block [ids | counts | dists] out through a pinned host mirror
+  // one device block [ptr | norm2 | elems]
   const size_t ptr_bytes = static_cast<size_t>(nq + 1) * 8, nrm_off = ptr_bytes,
                el_off = nrm_off + ((static_cast<size_t>(nq) * 4 + 7) & ~static_cast<size_t>(7));
   EPS_TRY(ix->s_sparse_q.reserve(el_off + qe.size() * 8));
@@ -895,39 +821,10 @@ int eps_search_sparse_batch(eps_index* h, int64_t nq, const int64_t* q_offsets, 
   EPS_CUDA(cudaMemcpyAsync(d_q, qp.data(), ptr_bytes, cudaMemcpyHostToDevice, ix->stream));
   EPS_CUDA(cudaMemcpyAsync(d_q + nrm_off, qn.data(), static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, ix->stream));
   if (!qe.empty()) EPS_CUDA(cudaMemcpyAsync(d_q + el_off, qe.data(), qe.size() * 8, cudaMemcpyHostToDevice, ix->stream));
-  const size_t n_ids = static_cast<size_t>(nq) * limit;
-  const size_t off_cnt = n_ids * 8, off_dist = off_cnt + static_cast<size_t>(nq) * 8, total = off_dist + n_ids * 4;
-  EPS_TRY(ix->s_out_ids.reserve(total));
-  if (ix->h_out_cap < total) {
-    if (ix->h_out) cudaFreeHost(ix->h_out);
-    ix->h_out = nullptr;
-    ix->h_out_cap = 0;
-    EPS_CUDA(cudaHostAlloc(&ix->h_out, total, cudaHostAllocDefault));
-    ix->h_out_cap = total;
-  }
-  unsigned char* d_blk = ix->s_out_ids.as<unsigned char>();
   const eps::SparseQueries q{reinterpret_cast<const int64_t*>(d_q), reinterpret_cast<const uint2*>(d_q + el_off),
                              reinterpret_cast<const float*>(d_q + nrm_off)};
-  EPS_TRY(eps::search_sparse_device(ix, q, nq, limit, filter, n_filter, reinterpret_cast<int64_t*>(d_blk),
-                                    reinterpret_cast<float*>(d_blk + off_dist), reinterpret_cast<int64_t*>(d_blk + off_cnt), stats));
-  EPS_CUDA(cudaMemcpyAsync(ix->h_out, d_blk, total, cudaMemcpyDeviceToHost, ix->stream));
-  if (stats) EPS_CUDA(cudaEventRecord(ix->ev[3], ix->stream));
-  EPS_CUDA(cudaStreamSynchronize(ix->stream));
-  const unsigned char* hb = static_cast<const unsigned char*>(ix->h_out);
-  std::memcpy(out_ids, hb, n_ids * 8);
-  std::memcpy(out_counts, hb + off_cnt, static_cast<size_t>(nq) * 8);
-  const float* hd = reinterpret_cast<const float*>(hb + off_dist);
-  for (size_t i = 0; i < n_ids; ++i) out_dists[i] = static_cast<double>(hd[i]);
-  if (stats) {
-    if (ix->graph_counters_pending) EPS_TRY(eps::read_graph_counters(ix, stats));
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, ix->ev[1], ix->ev[2]);
-    stats->kernel_ms += ms;
-    cudaEventElapsedTime(&ms, ix->ev[0], ix->ev[3]);
-    stats->total_ms += ms;
-  }
-  ix->graph_counters_pending = false;
-  return EPS_OK;
+  return eps::search_to_host(ix, eps::SparseBatch(q, nq, ix->metric), nq, limit, filter, n_filter, out_ids, out_dists,
+                             out_counts, stats);
 }
 
 int eps_merge_shards_device(int device, const int64_t* d_ids, const float* d_dists, int64_t n_shards, int64_t nq,

@@ -96,9 +96,6 @@ __global__ void facet_group_kernel(FacetArgs a) {
   if (lane == 0) a.out_groups[q] = ngroups;
 }
 
-int lower_filter(const eps_filter_node* nodes, int64_t n, FilterProg* out);
-int bind_program_columns(Index* ix, FilterProg* prog);
-
 }  // namespace eps
 
 using eps::Index;
@@ -114,11 +111,7 @@ extern "C" int eps_facet_batch(eps_index* h, const int64_t* ids, const double* d
   if (spec->key_type < 0 || spec->key_type > eps::VT_BOOL) return eps::fail(EPS_ERR_UNSUPPORTED, "group-by key must be string, int, double or bool");
   for (int64_t q = 0; q < nq; ++q)
     if (counts[q] < 0 || counts[q] > limit) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "result count outside [0, limit]");
-  {
-    int n = 0;
-    if (cudaGetDeviceCount(&n) != cudaSuccess || n <= 0) return eps::fail(EPS_ERR_NO_DEVICE, "no usable CUDA device (libepsilla_b200 has no CPU path)");
-    EPS_CUDA(cudaSetDevice(ix->device));
-  }
+  EPS_TRY(eps::check_device(ix->device));
   const int n_aggs = spec->n_aggs;
   std::vector<eps::FilterProg> progs(static_cast<size_t>(1 + n_aggs));
   EPS_TRY(eps::lower_filter(spec->key_nodes, spec->n_key_nodes, &progs[0]));

@@ -41,23 +41,14 @@ struct StrDict {
   int64_t bytes = 0, byte_cap = 0;
 };
 
-struct Index {
-  int device = 0;
-  int metric = EPS_METRIC_L2;
-  int64_t dim = 0;
+// Device data a base owns and its views alias; only the base frees it.
+struct Table {
   int64_t capacity = 0;
-  const float* host_vectors = nullptr;
   float* d_vectors = nullptr;   // [capacity x dim] (owned unless adopted)
-  bool owns_vectors = false;
-  Index* view_of = nullptr;     // read-only view (eps_index_create_view): table, graph, segment mirrors belong to this index
-  int n_views = 0;              // live views of this index; mutating entry points refuse while > 0
-  std::vector<Index*> views;    // the live views (detached when the base is destroyed first)
-  bool detached_view = false;   // a view whose base has been destroyed: holds no data any more
   int64_t n_rows = 0;           // rows mirrored so far (record_number_ snapshot)
   bool vec4 = false;            // dim % 4 == 0 and 16-B aligned base
 
   // sparse column (eps_index_create_sparse): rows are a CSR of {uint32 index, float value} elements
-  bool sparse = false;
   int64_t* d_sp_ptr = nullptr;  // [sp_row_cap + 1] element offsets of the rows
   uint2* d_sp_elems = nullptr;  // [sp_elem_cap] {index, value bits}, indices strictly increasing within a row
   float* d_sp_norm2 = nullptr;  // [sp_row_cap] sequential fp32 sum of squares of each row (cosine)
@@ -69,26 +60,33 @@ struct Index {
   int64_t nav = 0;
   int64_t* d_offsets = nullptr;  // [n_indexed + 1]
   int32_t* d_nbrs = nullptr;     // [n_edges]
-  int32_t* d_init_ids = nullptr; // seed set for init_L
-  int64_t init_L = 0;
   int32_t* d_ell = nullptr;      // fixed-stride adjacency [n_indexed x 64] (-1 padded), built lazily
-  int64_t seed_rows_L = 0;       // L for which s_seed_rows holds the gathered seed rows
 
   // segment mirrors
   uint8_t* d_deleted = nullptr;
   int64_t deleted_bytes = 0;
   int64_t deleted_cap = 0;
-  std::vector<uint8_t> h_deleted;  // host shadow of the uploaded bitset (dirty-span detection)
   bool any_deleted = false;
   char* d_attrs = nullptr;
   int64_t attr_stride = 0;
   int64_t attr_rows = 0;
   int64_t attr_cap_rows = 0;
-  const char* attr_src = nullptr;  // host table the mirror was filled from (append detection)
   StrCol str_cols[kMaxStringCols];
   StrDict dict;
 
-  // executor parameters
+  // principal-subspace sketch of the indexed rows (sketch.cu), computed when a graph is installed; a view shares its
+  // base's.  Dropped with the graph or the rows under it.
+  int sk_m = 0;                  // floats per row sketch: kSketch, or 0 while there is no basis
+  double sk_share = -1.0;        // share of the sampled variance the basis carries; -1 = no basis
+  float sk_g = 0.f;              // 1 - gamma_{m+2}, rounded down
+  float sk_scale = 0.f;          // (1 - 2 (dim + 2) 2^-24) / (1 + eps), rounded down
+  double sk_eps = 0.0;           // sigma_max(P~)^2 <= 1 + sk_eps
+  float* d_sk_basis = nullptr;   // [dim x sk_m] fp32 basis P~ (transposed), then [dim] mean
+  float* d_sk = nullptr;         // [n_indexed x sk_m] row sketches, then [n_indexed] their error bounds (null: screen off)
+};
+
+// Executor and tuning parameters: a view starts with its base's and sets its own afterwards.
+struct Config {
   int64_t L_master = 500, L_local = 500;
   bool prefilter = false;
   bool force_brute = false;
@@ -96,18 +94,38 @@ struct Index {
   int search_width = 1;          // candidates expanded per iteration (1 = the reference's sequential order)
   int graph_ring_slots = 0;      // row-ring slots per CTA of the graph kernel (0 = auto)
   int graph_ctas_per_sm = 0;     // cap on resident CTAs (= in-flight queries) per SM (0 = occupancy limit)
+  int coarse_mode = 1;           // exact-scan coarse pass: 0 = fp32 SIMT only, 1 = wgmma TF32, 2 = wgmma bf16 mirror
+  int coarse_guard = 1;          // verify the coarse pass after the re-score and redo unsafe queries (brute_force.cu)
+  int coarse_boost = 1;          // multiplier of k' learnt by the guard for this table (1, 4, 16, 64)
+  int graph_screen = EPS_GRAPH_SCREEN_AUTO;
+};
+
+struct Index : Table, Config {
+  int device = 0;
+  int metric = EPS_METRIC_L2;
+  int64_t dim = 0;
+  bool sparse = false;
+  int num_sms = 132;
+  const float* host_vectors = nullptr;
+  bool owns_vectors = false;
+  Index* view_of = nullptr;     // read-only view (eps_index_create_view): its Table belongs to this index
+  int n_views = 0;              // live views of this index; mutating entry points refuse while > 0
+  std::vector<Index*> views;    // the live views (detached when the base is destroyed first)
+  bool detached_view = false;   // a view whose base has been destroyed: holds no data any more
+  std::vector<uint8_t> h_deleted;  // host shadow of the uploaded deleted bitset (dirty-span detection)
+  const char* attr_src = nullptr;  // host table the attribute mirror was filled from (append detection)
+
+  int32_t* d_init_ids = nullptr; // seed set for init_L
+  int64_t init_L = 0;
+  int64_t seed_rows_L = 0;       // L for which s_seed_rows holds the gathered seed rows
 
   cudaStream_t stream = nullptr;
   cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-  int num_sms = 132;
 
   // scratch
   DevBuf s_queries, s_dist, s_topk, s_topk2, s_pass, s_filter, s_vset, s_visited, s_vlog, s_queue, s_tail, s_out_ids, s_out_dists,
       s_out_counts, s_stats, s_misc, s_seed_rows, s_seed_dist, s_xnorm, s_qnorm, s_coarse, s_thr, s_cand, s_cand_cnt, s_bf16, s_qbf16, s_flags,
       s_sparse_q, s_xnorm_max, s_like, s_like_jobs;
-  int coarse_mode = 1;           // exact-scan coarse pass: 0 = fp32 SIMT only, 1 = wgmma TF32, 2 = wgmma bf16 mirror
-  int coarse_guard = 1;          // verify the coarse pass after the re-score and redo unsafe queries (brute_force.cu)
-  int coarse_boost = 1;          // multiplier of k' learnt by the guard for this table (1, 4, 16, 64)
   int64_t bf16_rows = 0;
   const void* bf16_ptr = nullptr;
   int64_t xnorm_rows = 0;        // rows whose |x|^2 is current in s_xnorm; s_xnorm_max holds the largest (float bits)
@@ -122,17 +140,6 @@ struct Index {
   int64_t prof_nq = 0;           // developer build (EPS_GS_PROFILE): queries of the last profiled launch
   DevBuf s_prof_basis;           // developer build: principal subspace of the first prof_basis_rows rows (sketch.cu)
   int64_t prof_basis_rows = 0;
-
-  // principal-subspace sketch of the indexed rows (sketch.cu), computed when a graph is installed; a view shares its
-  // base's.  Dropped with the graph or the rows under it.
-  int graph_screen = EPS_GRAPH_SCREEN_AUTO;
-  int sk_m = 0;                  // floats per row sketch: kSketch, or 0 while there is no basis
-  double sk_share = -1.0;        // share of the sampled variance the basis carries; -1 = no basis
-  float sk_g = 0.f;              // 1 - gamma_{m+2}, rounded down
-  float sk_scale = 0.f;          // (1 - 2 (dim + 2) 2^-24) / (1 + eps), rounded down
-  double sk_eps = 0.0;           // sigma_max(P~)^2 <= 1 + sk_eps
-  float* d_sk_basis = nullptr;   // [dim x sk_m] fp32 basis P~ (transposed), then [dim] mean
-  float* d_sk = nullptr;         // [n_indexed x sk_m] row sketches, then [n_indexed] their error bounds (null: screen off)
   DevBuf s_qsk;                  // [nq x sk_m] query sketches, then [nq] their error bounds
   unsigned long long* d_screened = nullptr;  // device count of the fresh neighbours the screen dropped on this handle
   void* h_out = nullptr;         // pinned host mirror of the packed result block (eps_search_batch)
@@ -300,7 +307,10 @@ int check_like(const Index* ix, const FilterProg& prog);
 // *launches (if given) counts the launch.
 int bind_like(Index* ix, FilterProg* progs, int n, uint64_t* launches);
 
-// ---- misc kernels (capi.cu) ----------------------------------------------------------------
+// ---- capi.cu -------------------------------------------------------------------------------
 int normalize_rows_device(cudaStream_t s, float* d, int64_t n, int64_t dim);
+int check_device(int device);
+int bind_program_columns(Index* ix, FilterProg* prog);
+void free_graph(Index* ix);  // the graph, its seed set and everything derived from them
 
 }  // namespace eps

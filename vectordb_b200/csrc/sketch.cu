@@ -154,13 +154,13 @@ float round_down(double x) {
 }  // namespace
 
 void free_sketch_rows(Index* ix) {
-  if (!ix->view_of && !ix->detached_view && ix->d_sk) cudaFree(ix->d_sk);
+  if (ix->d_sk) cudaFree(ix->d_sk);
   ix->d_sk = nullptr;
 }
 
 void free_sketch(Index* ix) {
   free_sketch_rows(ix);
-  if (!ix->view_of && !ix->detached_view && ix->d_sk_basis) cudaFree(ix->d_sk_basis);
+  if (ix->d_sk_basis) cudaFree(ix->d_sk_basis);
   ix->d_sk_basis = nullptr;
   ix->sk_m = 0;
   ix->sk_share = -1.0;
@@ -234,7 +234,6 @@ int compute_sketch(Index* ix) {
 }  // namespace
 
 void ensure_sketch(Index* ix) {
-  if (ix->view_of || ix->detached_view) return;
   if (ix->metric != EPS_METRIC_L2 || ix->graph_screen == EPS_GRAPH_SCREEN_OFF || ix->dim < 128 || ix->n_indexed < 1 ||
       !ix->d_vectors) {
     free_sketch_rows(ix);

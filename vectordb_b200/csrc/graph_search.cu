@@ -65,8 +65,8 @@ constexpr int kMaxR = 24;       // ring slots (upper bound: 3 consumer warps x k
 constexpr int kRounds = kMaxW * kEll / kGsThreads;  // adjacency slots per thread
 
 // Developer build only (make EXTRA=-DEPS_GS_PROFILE): per-phase cycle counters of warp 0 (pick / adjacency / merge /
-// barrier waits) and of warp 1 (row wait / row math), summed over CTAs into stats[8..23], and the prefix-rejection
-// counts of prof_prefix_fails in stats[25..29] and of prof_sketch_fails in stats[32..33].  Compiled out otherwise.
+// barrier waits) and of warp 1 (row wait / row math), summed over CTAs into the kGcPhase slots of the counter block, the
+// visited-set counts and a per-query timeline.  Compiled out otherwise.
 #ifdef EPS_GS_PROFILE
 #define GS_T(var) const long long var = clock64()
 #define GS_ACC(slot, t0, t1) do { if (lane == 0) prof[slot] += (t1) - (t0); } while (0)
@@ -92,16 +92,16 @@ struct GSArgs {
   int vlog_cap;
   unsigned long long* out_queue;  // [nq x L]
   int* work_counter;
-  unsigned long long* stats;      // n_dist, n_expand, n_edges (+ developer counters, see read_graph_counters)
+  unsigned long long* stats;      // counter block (GraphCounter slots)
   int64_t visited_words;
   int64_t seed_ld;
-  int dim, metric, vec4;
+  int dim, metric, vec4;  // vec4: not read; removing it, or moving qtimes, grows the spills of the 72- and 128-register instances
   int L, Lp;
   int nq;
   int W;                          // candidates per iteration (the search width)
   int R;                          // ring slots (slot s is owned by consumer warp s % 3)
   int fc;                         // fresh-id FIFO capacity (power of two)
-  unsigned long long* qtimes;     // developer build: [nq x 2] globaltimer at query start / end (null otherwise)
+  unsigned long long* qtimes;     // developer build: [nq x 4] globaltimer at query start and end, n_dist, iterations
   int slot_bytes;                 // ring slot pitch (row bytes, multiple of 16); 0 when rows are not staged
   // screen (sketch.cu; sk == null: off): fresh neighbours whose sketch bound fails the bound never enter the FIFO
   const float* sk;                // [n x kSketch] row sketches, then [n] their error bounds
@@ -109,10 +109,6 @@ struct GSArgs {
   int64_t n_sk;                   // rows sketched (n_indexed)
   float sk_g, sk_scale;           // rounded-down factors of the bound (see screen_fresh)
   unsigned long long* n_screened; // ids the screen dropped, summed over every search of the handle
-#ifdef EPS_GS_PROFILE
-  const float* prof_basis;        // [prof_m x dim] principal subspace of the table (null: not counted)
-  int prof_m;
-#endif
 };
 
 template <bool L2>
@@ -163,77 +159,6 @@ __device__ __forceinline__ void warp_rows_scalar(const float* const (&rows)[S], 
 #pragma unroll
   for (int s = 0; s < S; ++s) out[s] = warp_sum(acc[s]);
 }
-
-#ifdef EPS_GS_PROFILE
-// Developer build: could a prefix of a staged L2 row reject it before the rest is read?  For t = dim4 * j / 4 float4
-// chunks (j = 1..4; j = 4 is the whole row), cnt[j] counts the rows of `mask` whose prefix already fails the bound.  The
-// test is the exact one a prefix rejection would need: lane l's chain over its chunks l, l + 32, ... below t is an
-// intermediate value of its full fmaf chain, each step adds a square >= 0, so lane s's butterfly of the partial chains
-// is <= its distance of row s, and a partial key >= bound proves that the full key fails too.  A second pass over the
-// rows in shared memory: the distances the search uses are untouched.
-template <int S>
-__device__ __forceinline__ void prof_prefix_fails(const unsigned char* first, uint32_t step, unsigned mask, const float4* q, int dim4,
-                                                  int lane, const int* slot_id, int cw, unsigned long long bound,
-                                                  unsigned long long* cnt) {
-  if (lane < S && ((mask >> lane) & 1u)) ++cnt[0];
-  for (int j = 1; j <= 4; ++j) {
-    const int t = dim4 * j / 4;
-    float acc[S];
-#pragma unroll
-    for (int s = 0; s < S; ++s) acc[s] = 0.f;
-    for (int c = lane; c < t; c += 32) {
-      const float4 y = q[c];
-#pragma unroll
-      for (int s = 0; s < S; ++s)
-        if ((mask >> s) & 1u) acc4<true>(reinterpret_cast<const float4*>(first + s * step)[c], y, acc[s]);
-    }
-#pragma unroll
-    for (int s = 0; s < S; ++s) {
-      const float v = warp_sum(acc[s]);
-      if (lane == s && ((mask >> s) & 1u) && make_key(v, static_cast<uint32_t>(slot_id[cw + 3 * s])) >= bound) ++cnt[j];
-    }
-  }
-}
-
-// Developer build: could a lower bound from the table's principal subspace reject a staged L2 row before the row is
-// read?  P [m x dim4 float4] has orthonormal rows (sketch.cu), so |P(x - q)|^2 <= |x - q|^2; cnt[0] / cnt[1] count the
-// rows for which the bound of the first 32 / all m rows of P, shrunk by 1e-3 to cover the rounding of both sides
-// (a bound held to the kernel's fp32 sum needs about 1e-4 at d = 768), already fails the bound of the consumer.
-template <int S>
-__device__ __forceinline__ void prof_sketch_fails(const unsigned char* first, uint32_t step, unsigned mask, const float4* q, int dim4,
-                                                  int lane, const int* slot_id, int cw, unsigned long long bound,
-                                                  const float4* __restrict__ P, int m, unsigned long long* cnt) {
-  float acc[S];
-#pragma unroll
-  for (int s = 0; s < S; ++s) acc[s] = 0.f;
-  for (int j = 0; j < m; ++j) {
-    float part[S];
-#pragma unroll
-    for (int s = 0; s < S; ++s) part[s] = 0.f;
-    for (int c = lane; c < dim4; c += 32) {
-      const float4 p = __ldg(P + static_cast<size_t>(j) * dim4 + c), y = q[c];
-#pragma unroll
-      for (int s = 0; s < S; ++s)
-        if ((mask >> s) & 1u) {
-          const float4 x = reinterpret_cast<const float4*>(first + s * step)[c];
-          part[s] += p.x * (x.x - y.x) + p.y * (x.y - y.y) + p.z * (x.z - y.z) + p.w * (x.w - y.w);
-        }
-    }
-#pragma unroll
-    for (int s = 0; s < S; ++s) {
-      const float v = warp_sum(part[s]);
-      acc[s] = fmaf(v, v, acc[s]);
-    }
-    if (j == 31 || j == m - 1) {
-#pragma unroll
-      for (int s = 0; s < S; ++s)
-        if (lane == s && ((mask >> s) & 1u) &&
-            make_key(acc[s] * (1.f - 1e-3f), static_cast<uint32_t>(slot_id[cw + 3 * s])) >= bound)
-          ++cnt[j == m - 1 ? 1 : 0];
-    }
-  }
-}
-#endif
 
 // Screen of the fresh ids fifo[tail .. tail + total) of one expansion step (all 128 threads).  Eight lanes per id read its
 // sketch s_x (one float4 each) and its error bound ex_x; the loads of up to kScreenIds ids are issued before any is
@@ -295,8 +220,7 @@ __device__ __forceinline__ void screen_fresh(const GSArgs& a, const int* fifo, u
 template <int S>
 __device__ __forceinline__ void consume_slots(const GSArgs& a, unsigned occ_mask, unsigned par_mask, int cw, int lane, bool staged,
                                               const unsigned char* ring, uint32_t bar0, const float* qv, const int* slot_id,
-                                              unsigned long long bound, unsigned long long* pend, int* s_npend,
-                                              unsigned long long* prefix_cnt) {
+                                              unsigned long long bound, unsigned long long* pend, int* s_npend) {
   float d[S];
   if (staged) {
 #pragma unroll
@@ -306,13 +230,6 @@ __device__ __forceinline__ void consume_slots(const GSArgs& a, unsigned occ_mask
     const uint32_t step = 3u * static_cast<uint32_t>(a.slot_bytes);
     if (a.metric == EPS_METRIC_L2) warp_rows_vec4<true, S>(first, step, occ_mask, reinterpret_cast<const float4*>(qv), a.dim >> 2, lane, d);
     else warp_rows_vec4<false, S>(first, step, occ_mask, reinterpret_cast<const float4*>(qv), a.dim >> 2, lane, d);
-#ifdef EPS_GS_PROFILE
-    if (a.metric == EPS_METRIC_L2)
-      prof_prefix_fails<S>(first, step, occ_mask, reinterpret_cast<const float4*>(qv), a.dim >> 2, lane, slot_id, cw, bound, prefix_cnt);
-    if (a.metric == EPS_METRIC_L2 && a.prof_basis)
-      prof_sketch_fails<S>(first, step, occ_mask, reinterpret_cast<const float4*>(qv), a.dim >> 2, lane, slot_id, cw, bound,
-                           reinterpret_cast<const float4*>(a.prof_basis), a.prof_m, prefix_cnt + 5);
-#endif
   } else {
     const float* rows[S];
 #pragma unroll
@@ -384,12 +301,7 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
 #ifdef EPS_GS_PROFILE
   long long prof[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // 0 barrier X, 1 merge, 2 row wait, 3 row math, 4 pick, 5 barrier 1, 6 adjacency+visited, 7 barrier 2 + FIFO
   const long long t_kernel0 = clock64();
-  // staged L2 rows evaluated; of them, rows whose 1/4 .. 4/4 prefix fails the bound; rows whose 32- / m-float sketch
-  // bound fails it
-  unsigned long long prefix_cnt[7] = {0, 0, 0, 0, 0, 0, 0};
   unsigned long long prof_vtest = 0, prof_migrated = 0;  // hash-set test-and-inserts of this thread; queries moved to the bitmap
-#else
-  unsigned long long* prefix_cnt = nullptr;
 #endif
 
   for (;;) {
@@ -399,7 +311,7 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
     const int q = s_q;
     if (q >= a.nq) break;
 #ifdef EPS_GS_PROFILE
-    if (tid == 0 && a.qtimes) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); a.qtimes[4 * q] = t; }
+    if (tid == 0) { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); a.qtimes[4 * q] = t; }
     const unsigned long long prof_nd0 = st_ndist;
     unsigned long long prof_iters = 0;
 #endif
@@ -473,10 +385,10 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
         for (;;) {
           if (occ_mask) {
             GS_T(tw0);
-            if (n_own <= 1) consume_slots<1>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend, prefix_cnt);
-            else if (n_own <= 2) consume_slots<2>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend, prefix_cnt);
-            else if (n_own <= 4) consume_slots<4>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend, prefix_cnt);
-            else consume_slots<8>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend, prefix_cnt);
+            if (n_own <= 1) consume_slots<1>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend);
+            else if (n_own <= 2) consume_slots<2>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend);
+            else if (n_own <= 4) consume_slots<4>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend);
+            else consume_slots<8>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend);
             par_mask ^= occ_mask;
             GS_T(tw1);
             GS_ACC(3, tw0, tw1);
@@ -765,7 +677,7 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
     unsigned long long* out = a.out_queue + static_cast<int64_t>(q) * L;
     for (int i = tid; i < L; i += kGsThreads) out[i] = qa[i];
 #ifdef EPS_GS_PROFILE
-    if (tid == 0 && a.qtimes) {
+    if (tid == 0) {
       unsigned long long t;
       asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
       a.qtimes[4 * q + 1] = t; a.qtimes[4 * q + 2] = st_ndist - prof_nd0; a.qtimes[4 * q + 3] = prof_iters;
@@ -795,18 +707,16 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
   }
 #ifdef EPS_GS_PROFILE
   if (lane == 0 && warp < 2) {
-    for (int i = 0; i < 8; ++i) atomicAdd(&a.stats[8 + warp * 8 + i], static_cast<unsigned long long>(prof[i]));
-    if (warp == 0) atomicAdd(&a.stats[24], static_cast<unsigned long long>(clock64() - t_kernel0));
+    for (int i = 0; i < 8; ++i) atomicAdd(&a.stats[kGcPhase + warp * 8 + i], static_cast<unsigned long long>(prof[i]));
+    if (warp == 0) atomicAdd(&a.stats[kGcCycles], static_cast<unsigned long long>(clock64() - t_kernel0));
   }
-  for (int i = 0; i < 5; ++i) if (prefix_cnt[i]) atomicAdd(&a.stats[25 + i], prefix_cnt[i]);
-  for (int i = 0; i < 2; ++i) if (prefix_cnt[5 + i]) atomicAdd(&a.stats[32 + i], prefix_cnt[5 + i]);
-  if (prof_vtest) atomicAdd(&a.stats[5], prof_vtest);
-  if (prof_migrated) atomicAdd(&a.stats[30], prof_migrated);
-  if (vacc) atomicAdd(&a.stats[31], vacc);
+  if (prof_vtest) atomicAdd(&a.stats[kGcVsetTests], prof_vtest);
+  if (prof_migrated) atomicAdd(&a.stats[kGcMigrated], prof_migrated);
+  if (vacc) atomicAdd(&a.stats[kGcVsetAccesses], vacc);
 #endif
-  if (st_ndist) atomicAdd(&a.stats[0], st_ndist);
-  if (st_nexp) atomicAdd(&a.stats[1], st_nexp);
-  if (st_nedge) atomicAdd(&a.stats[2], st_nedge);
+  if (st_ndist) atomicAdd(&a.stats[kGcDist], st_ndist);
+  if (st_nexp) atomicAdd(&a.stats[kGcExpand], st_nexp);
+  if (st_nedge) atomicAdd(&a.stats[kGcEdges], st_nedge);
   if (st_nscr) atomicAdd(a.n_screened, st_nscr);
 }
 
@@ -897,10 +807,8 @@ int ensure_ell(Index* ix, uint64_t* launches) {
 
 int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsigned long long* d_queue,
                  eps_stats* stats) {
-  if (L < 1 || L > ix->n_indexed) return fail(EPS_ERR_INVALID_ARGUMENT, "graph_search: L out of range");
-  const int Lp = std::max(2, next_pow2(static_cast<int>(L)));
-  if (Lp > 16384) return fail(EPS_ERR_UNSUPPORTED, "SearchQueueSize above 16384 is not supported by the graph kernel");
-  EPS_TRY(prepare_init_ids(ix, L));
+  int Lp = 0;
+  EPS_TRY(graph_launch_prologue(ix, L, "graph_search", &Lp));
   const int dim = static_cast<int>(ix->dim);
   const int dimp = (dim + 3) & ~3;
   const int width = std::max(1, std::min(ix->search_width, kMaxW));
@@ -948,9 +856,7 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
     slots = static_cast<int>(std::min<int64_t>(nq, static_cast<int64_t>(per_sm) * ix->num_sms));
   VisitedSets vis;
   EPS_TRY(prepare_visited(ix, slots, L, &vis));
-  EPS_TRY(ix->s_misc.reserve(512));  // [0..3] counters, [+32 B] work counter, [5] [30..31] developer hash-set counts,
-                                     // [8..24] developer phase timers, [25..29] [32..33] developer prefix / sketch counts
-  EPS_CUDA(cudaMemsetAsync(ix->s_misc.p, 0, 512, ix->stream));
+  EPS_TRY(graph_counters(ix, nq));
   uint64_t launches = 1;
   EPS_TRY(ensure_ell(ix, &launches));
   if (ix->seed_rows_L != L) {  // contiguous copy of the query-independent seed rows
@@ -972,7 +878,7 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   a.vlog = vis.vlog; a.vlog_cap = vis.vlog_cap;
   a.vset = vis.vset; a.vset_cap = vis.vset_cap; a.vset_max = vis.vset_max; a.vset_shift = vis.vset_shift;
   a.visited = vis.visited; a.out_queue = d_queue;
-  a.work_counter = reinterpret_cast<int*>(ix->s_misc.as<unsigned char>() + 32);
+  a.work_counter = reinterpret_cast<int*>(ix->s_misc.as<unsigned long long>() + kGcWork);
   a.stats = ix->s_misc.as<unsigned long long>();
   a.visited_words = vis.words; a.seed_ld = seed_ld; a.dim = dim; a.metric = ix->metric;
   a.vec4 = ix->vec4 ? 1 : 0; a.L = static_cast<int>(L); a.Lp = Lp; a.nq = static_cast<int>(nq);
@@ -993,25 +899,9 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   }
 
 #ifdef EPS_GS_PROFILE
-  EPS_TRY(ix->s_tail.reserve(static_cast<size_t>(nq) * 32));  // borrowed scratch (the hybrid tail buffer is filled after the search)
-  a.qtimes = ix->s_tail.as<unsigned long long>();
-  ix->prof_nq = nq;
-  a.prof_basis = nullptr;
-  a.prof_m = 64;
-  if (ix->metric == EPS_METRIC_L2 && staged && dim >= a.prof_m) {
-    if (ix->prof_basis_rows != ix->n_indexed) {
-      std::vector<float> basis, mean;
-      double share = 0;
-      EPS_TRY(principal_subspace(ix, a.prof_m, &basis, &mean, &share));
-      EPS_TRY(ix->s_prof_basis.reserve(basis.size() * 4));
-      EPS_CUDA(cudaMemcpyAsync(ix->s_prof_basis.p, basis.data(), basis.size() * 4, cudaMemcpyHostToDevice, ix->stream));
-      EPS_CUDA(cudaStreamSynchronize(ix->stream));
-      ix->prof_basis_rows = ix->n_indexed;
-      fprintf(stderr, "[gs-profile] principal subspace of %lld rows: the top %d components carry %.4f of the variance\n",
-              static_cast<long long>(ix->n_indexed), a.prof_m, share);
-    }
-    a.prof_basis = ix->s_prof_basis.as<float>();
-  }
+  EPS_TRY(ix->s_prof_qtimes.reserve(static_cast<size_t>(nq) * 32));
+  a.qtimes = ix->s_prof_qtimes.as<unsigned long long>();
+  ix->prof_timeline = true;
 #endif
   // at most 4 resident CTAs per SM (what the auto rule picks for batches above one wave at 7 per SM, e.g. 1024 queries
   // at L = 768): the register file has room for 128 registers per thread, so the instance that hardly spills runs;
@@ -1025,6 +915,23 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
     stats->n_seed += static_cast<uint64_t>(nq) * static_cast<uint64_t>(L);
     stats->kernel_launches += launches;
   }
+  return EPS_OK;
+}
+
+int graph_launch_prologue(Index* ix, int64_t L, const char* who, int* Lp) {
+  if (L < 1 || L > ix->n_indexed) return fail(EPS_ERR_INVALID_ARGUMENT, std::string(who) + ": L out of range");
+  *Lp = std::max(2, next_pow2(static_cast<int>(L)));
+  if (*Lp > 16384) return fail(EPS_ERR_UNSUPPORTED, "SearchQueueSize above 16384 is not supported by the graph kernel");
+  return prepare_init_ids(ix, L);
+}
+
+int graph_counters(Index* ix, int64_t nq) {
+  EPS_TRY(ix->s_misc.reserve(kGcSlots * 8));
+  EPS_CUDA(cudaMemsetAsync(ix->s_misc.p, 0, kGcSlots * 8, ix->stream));
+#ifdef EPS_GS_PROFILE
+  ix->prof_nq = nq;
+  ix->prof_timeline = false;  // graph_search sets up a per-query timeline
+#endif
   return EPS_OK;
 }
 
@@ -1066,40 +973,26 @@ int prepare_visited(Index* ix, int slots, int64_t L, VisitedSets* v) {
 // Device counters of the last graph_search launch (call after the stream has been synchronised).
 int read_graph_counters(Index* ix, eps_stats* stats) {
   if (!stats || !ix->s_misc.p) return EPS_OK;
-  unsigned long long h[4];
-  EPS_CUDA(cudaMemcpy(h, ix->s_misc.p, 32, cudaMemcpyDeviceToHost));
-  stats->n_dist += h[0];
-  stats->n_expand += h[1];
-  stats->n_edges += h[2];
+  unsigned long long h[kGcSlots];
+  EPS_CUDA(cudaMemcpy(h, ix->s_misc.p, sizeof(h), cudaMemcpyDeviceToHost));
+  stats->n_dist += h[kGcDist];
+  stats->n_expand += h[kGcExpand];
+  stats->n_edges += h[kGcEdges];
 #ifdef EPS_GS_PROFILE
-  unsigned long long pr[64];
-  EPS_CUDA(cudaMemcpy(pr, ix->s_misc.p, 512, cudaMemcpyDeviceToHost));
+  const unsigned long long* pr = h;
   const char* names[8] = {"barrierX", "merge", "row_wait", "team_phase", "pick", "barrier1", "adj+visited", "barrier2+fifo"};
-  const double tot = static_cast<double>(pr[24]) + 1.0;
+  const double tot = static_cast<double>(pr[kGcCycles]) + 1.0;
   fprintf(stderr, "[gs-profile] kernel cycles summed over CTAs %.3e;", tot);
   for (int w = 0; w < 2; ++w)
-    for (int i = 0; i < 8; ++i) fprintf(stderr, " w%d.%s=%.1f%%", w, names[i], 100.0 * static_cast<double>(pr[8 + w * 8 + i]) / tot);
+    for (int i = 0; i < 8; ++i) fprintf(stderr, " w%d.%s=%.1f%%", w, names[i], 100.0 * static_cast<double>(pr[kGcPhase + w * 8 + i]) / tot);
   fprintf(stderr, "\n");
   fprintf(stderr, "[gs-profile] visited hash set: %llu test-and-inserts, %.3f table accesses (bucket reads + CAS) each; "
                   "%llu queries moved to the bitmap (%.2f%%)\n",
-          pr[5], static_cast<double>(pr[31]) / (static_cast<double>(pr[5]) + 1e-9), pr[30],
-          ix->prof_nq > 0 ? 100.0 * static_cast<double>(pr[30]) / static_cast<double>(ix->prof_nq) : 0.0);
-  if (pr[25]) {
-    // fetching a prefix s of every row and the rest only where the prefix cannot reject it would stage
-    // s + (1 - p(s)) (1 - s) of the row bytes, p(s) = share of rows whose prefix s fails the bound
-    fprintf(stderr, "[gs-profile] staged L2 rows evaluated %llu; share whose prefix fails the bound (row bytes staged by a split there):", pr[25]);
-    for (int j = 1; j <= 4; ++j) {
-      const double p = static_cast<double>(pr[25 + j]) / static_cast<double>(pr[25]), s = 0.25 * j;
-      fprintf(stderr, " %d/4 %.4f (%.4f)", j, p, s + (1.0 - p) * (1.0 - s));
-    }
-    fprintf(stderr, "\n");
-    // fetching a sketch of b bytes for every evaluated row and the row only where the sketch cannot reject it
-    fprintf(stderr, "[gs-profile] share of those rows whose principal-subspace bound fails the bound: 32 floats %.4f, 64 floats %.4f\n",
-            static_cast<double>(pr[32]) / static_cast<double>(pr[25]), static_cast<double>(pr[33]) / static_cast<double>(pr[25]));
-  }
-  if (ix->prof_nq > 0 && ix->s_tail.p) {
+          pr[kGcVsetTests], static_cast<double>(pr[kGcVsetAccesses]) / (static_cast<double>(pr[kGcVsetTests]) + 1e-9), pr[kGcMigrated],
+          ix->prof_nq > 0 ? 100.0 * static_cast<double>(pr[kGcMigrated]) / static_cast<double>(ix->prof_nq) : 0.0);
+  if (ix->prof_timeline && ix->prof_nq > 0) {
     std::vector<unsigned long long> t(static_cast<size_t>(ix->prof_nq) * 4);
-    EPS_CUDA(cudaMemcpy(t.data(), ix->s_tail.p, t.size() * 8, cudaMemcpyDeviceToHost));
+    EPS_CUDA(cudaMemcpy(t.data(), ix->s_prof_qtimes.p, t.size() * 8, cudaMemcpyDeviceToHost));
     unsigned long long t0 = ~0ull, t1 = 0;
     for (int64_t q = 0; q < ix->prof_nq; ++q) { t0 = std::min(t0, t[4 * q]); t1 = std::max(t1, t[4 * q + 1]); }
     std::vector<double> end, dur;

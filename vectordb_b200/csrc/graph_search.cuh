@@ -1,5 +1,5 @@
-// Device code shared by the graph-search kernels (graph_search.cu: dense rows, sparse_graph.cu: sparse rows): the
-// visited hash set and the block merge of accepted keys into the sorted queue.
+// Device code shared by the graph-search kernels (graph_search.cu: dense rows, sparse_graph.cu: sparse rows): the slots
+// of their counter block, the visited hash set and the block merge of accepted keys into the sorted queue.
 #pragma once
 #include "common.cuh"
 
@@ -7,6 +7,19 @@ namespace eps {
 
 constexpr int kGsThreads = 128;
 constexpr int kPC = 128;        // accepted keys pending their merge (= one key per thread in the merge)
+
+// Counter block of one launch of either kernel (Index::s_misc, zeroed by graph_counters): 64-bit slots summed over CTAs.
+// read_graph_counters adds the first three to eps_stats; the developer build (EPS_GS_PROFILE) prints the others.
+enum GraphCounter {
+  kGcDist, kGcExpand, kGcEdges,  // n_dist, n_expand, n_edges
+  kGcWork,                       // work counter: the next query to claim (an int)
+  kGcVsetTests,                  // developer: hash-set test-and-inserts (dense kernel)
+  kGcVsetAccesses,               // developer: hash-set accesses (bucket reads + CAS)
+  kGcMigrated,                   // developer: queries moved to the bitmap (dense kernel)
+  kGcCycles,                     // developer: kernel cycles of warp 0 (dense kernel)
+  kGcPhase,                      // developer: 16 phase timers of the dense kernel, warp 0 then warp 1
+  kGcSlots = kGcPhase + 16
+};
 
 __device__ __forceinline__ int lb_masked(const unsigned long long* a, int n, unsigned long long key) {
   int lo = 0, hi = n;

@@ -137,9 +137,9 @@ struct Index : Table, Config {
   const void* vset_clean_ptr = nullptr;  // visited hash-set buffer known to be all-ones (empty), and its capacity
   size_t vset_clean_cap = 0;
   bool graph_counters_pending = false;
-  int64_t prof_nq = 0;           // developer build (EPS_GS_PROFILE): queries of the last profiled launch
-  DevBuf s_prof_basis;           // developer build: principal subspace of the first prof_basis_rows rows (sketch.cu)
-  int64_t prof_basis_rows = 0;
+  int64_t prof_nq = 0;           // developer build (EPS_GS_PROFILE): queries of the last graph-search launch
+  DevBuf s_prof_qtimes;          // developer build: [prof_nq x 4] per-query timeline of the last dense launch
+  bool prof_timeline = false;    // developer build: s_prof_qtimes belongs to the last launch
   DevBuf s_qsk;                  // [nq x sk_m] query sketches, then [nq] their error bounds
   unsigned long long* d_screened = nullptr;  // device count of the fresh neighbours the screen dropped on this handle
   void* h_out = nullptr;         // pinned host mirror of the packed result block (eps_search_batch)
@@ -221,6 +221,11 @@ int sparse_graph_search(Index* ix, const SparseQueries& q, int64_t nq, int64_t L
 int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsigned long long* d_queue,
                  eps_stats* stats);
 int prepare_init_ids(Index* ix, int64_t L);
+// Launch prologue shared by graph_search and sparse_graph_search: L in [1, n_indexed] (`who` names the caller in the
+// error), the padded queue length Lp (a power of two >= 2, at most 16384) and the init ids.
+int graph_launch_prologue(Index* ix, int64_t L, const char* who, int* Lp);
+// Reserves and zeroes the counter block of a launch of nq queries (graph_search.cuh, GraphCounter).
+int graph_counters(Index* ix, int64_t nq);
 int ensure_ell(Index* ix, uint64_t* launches);  // fixed-stride adjacency of the installed graph (built once)
 // out[i] = row d_ids[i] of the table (contiguous copy; used for seed rows and for the build's repair searches)
 int gather_rows(Index* ix, const int32_t* d_ids, int64_t n, float* d_out);

@@ -50,7 +50,7 @@ struct SGArgs {
   int vlog_cap;
   unsigned long long* out_queue;  // [nq x L]
   int* work_counter;
-  unsigned long long* stats;      // n_dist, n_expand, n_edges
+  unsigned long long* stats;      // counter block (GraphCounter slots)
   int L, Lp, nq;
 };
 
@@ -295,20 +295,18 @@ __global__ void __launch_bounds__(kGsThreads) sparse_graph_search_kernel(SGArgs 
     }
   }
 #ifdef EPS_GS_PROFILE
-  if (vacc) atomicAdd(&a.stats[31], vacc);
+  if (vacc) atomicAdd(&a.stats[kGcVsetAccesses], vacc);
 #endif
-  if (st_ndist) atomicAdd(&a.stats[0], st_ndist);
-  if (st_nexp) atomicAdd(&a.stats[1], st_nexp);
-  if (st_nedge) atomicAdd(&a.stats[2], st_nedge);
+  if (st_ndist) atomicAdd(&a.stats[kGcDist], st_ndist);
+  if (st_nexp) atomicAdd(&a.stats[kGcExpand], st_nexp);
+  if (st_nedge) atomicAdd(&a.stats[kGcEdges], st_nedge);
 }
 
 int sparse_graph_search(Index* ix, const SparseQueries& q, int64_t nq, int64_t L, unsigned long long* d_queue,
                         eps_stats* stats) {
-  if (L < 1 || L > ix->n_indexed) return fail(EPS_ERR_INVALID_ARGUMENT, "sparse_graph_search: L out of range");
+  int Lp = 0;
+  EPS_TRY(graph_launch_prologue(ix, L, "sparse_graph_search", &Lp));
   if (nq > INT_MAX) return fail(EPS_ERR_UNSUPPORTED, "sparse graph search: too many queries in one launch");
-  const int Lp = std::max(2, next_pow2(static_cast<int>(L)));
-  if (Lp > 16384) return fail(EPS_ERR_UNSUPPORTED, "SearchQueueSize above 16384 is not supported by the graph kernel");
-  EPS_TRY(prepare_init_ids(ix, L));
   const size_t smem = static_cast<size_t>(Lp) * 8 + 2 * kPC * 8 + static_cast<size_t>(kSgQCap) * 8 + kPC * 4 + kGsThreads * 4 +
                       static_cast<size_t>((Lp + 31) / 32) * 4;
   void (*kernel)(SGArgs) = ix->metric == EPS_METRIC_L2 ? sparse_graph_search_kernel<EPS_METRIC_L2>
@@ -321,8 +319,7 @@ int sparse_graph_search(Index* ix, const SparseQueries& q, int64_t nq, int64_t L
   const int slots = static_cast<int>(std::min<int64_t>(nq, static_cast<int64_t>(per_sm) * ix->num_sms));
   VisitedSets vis;
   EPS_TRY(prepare_visited(ix, slots, L, &vis));
-  EPS_TRY(ix->s_misc.reserve(256));  // [0..2] counters, [+32 B] work counter (read_graph_counters)
-  EPS_CUDA(cudaMemsetAsync(ix->s_misc.p, 0, 256, ix->stream));
+  EPS_TRY(graph_counters(ix, nq));
   SGArgs a;
   a.row_ptr = ix->d_sp_ptr; a.elems = ix->d_sp_elems; a.row_norm2 = ix->d_sp_norm2;
   a.offsets = ix->d_offsets; a.nbrs = ix->d_nbrs; a.init_ids = ix->d_init_ids;
@@ -330,7 +327,7 @@ int sparse_graph_search(Index* ix, const SparseQueries& q, int64_t nq, int64_t L
   a.vset = vis.vset; a.vset_cap = vis.vset_cap; a.vset_shift = vis.vset_shift; a.vset_max = vis.vset_max;
   a.visited = vis.visited; a.visited_words = vis.words; a.vlog = vis.vlog; a.vlog_cap = vis.vlog_cap;
   a.out_queue = d_queue;
-  a.work_counter = reinterpret_cast<int*>(ix->s_misc.as<unsigned char>() + 32);
+  a.work_counter = reinterpret_cast<int*>(ix->s_misc.as<unsigned long long>() + kGcWork);
   a.stats = ix->s_misc.as<unsigned long long>();
   a.L = static_cast<int>(L); a.Lp = Lp; a.nq = static_cast<int>(nq);
   kernel<<<slots, kGsThreads, smem, ix->stream>>>(a);

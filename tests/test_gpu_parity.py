@@ -418,6 +418,31 @@ def test_nn_descent_build_vs_reference_graph(vdb, golden_refgraph):
     ix.close()
 
 
+@pytest.mark.parametrize("m,below", [("l2", 60000), ("ip", 60000), ("ip", 1000)])
+def test_build_ignores_deleted_rows(vdb, m, below):
+    """The build indexes every row, deleted or not (ann_graph_segment.cpp:201): a deleted bitset leaves offsets,
+    neighbours and nav unchanged, on the exact-kNN branch and on the NN-descent branch (exact_knn_below under n, where
+    the navigation point's scan is the only one that could read the bits).  The bitset deletes the navigation point
+    itself, so a scan that skipped deleted rows would pick another; the inner-product cases cover that L2 scan on a
+    non-L2 field."""
+    n, d = 6000, 32
+    X = gen(n, d, 931, "cluster")
+    ix = vdb.Index(m, d, host_vectors=X)
+    ix.sync_rows(n)
+    ix.build(n, exact_knn_below=below)
+    want = ix.get_graph()
+    bits = np.zeros(n // 8 + 1, np.uint8)
+    bits[::3] = 0xA5
+    nav = want[3]
+    bits[nav >> 3] |= 1 << (nav & 7)
+    ix.set_deleted(bits)
+    ix.build(n, exact_knn_below=below)
+    got = ix.get_graph()
+    for name, a, b in zip(("n_indexed", "offsets", "neighbours", "nav"), got, want):
+        assert np.array_equal(a, b), name
+    ix.close()
+
+
 def test_build_repair_does_not_grow_hubs(vdb):
     """B2 connectivity repair (nsg.cpp:734-775: nearest linked vertex of a search pool, else a random linked one) on
     the case that used to produce one vertex of degree O(n): an inner-product field over positive data."""

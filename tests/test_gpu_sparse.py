@@ -336,3 +336,25 @@ def test_sparse_graph_build(vdb):
     Dq = ref_distances(R, densify(qs, vocab), IP)
     assert_bitwise(ix.search(qs, 10), ref_search(Dq, 10, 10), "search with a graph installed")
     ix.close()
+
+
+@pytest.mark.parametrize("metric", ["ip", "l2"])
+def test_sparse_graph_build_ignores_deleted_rows(vdb, metric):
+    """The sparse build indexes every row, deleted or not: a deleted bitset leaves the kNN lists and the L2 navigation
+    point unchanged.  The bitset deletes the navigation point itself, so a scan that skipped deleted rows would pick
+    another."""
+    n, vocab = 3000, 2000
+    rows = sparse_rows(n, vocab, 43)
+    ix = vdb.SparseIndex(metric, vocab)
+    ix.append(rows)
+    ix.build(n)
+    want = ix.get_graph()
+    bits = np.full(n // 8 + 1, 0x5A, np.uint8)
+    nav = want[3]
+    bits[nav >> 3] |= 1 << (nav & 7)
+    ix.set_deleted(bits)
+    ix.build(n)
+    got = ix.get_graph()
+    for name, a, b in zip(("n_indexed", "offsets", "neighbours", "nav"), got, want):
+        assert np.array_equal(a, b), name
+    ix.close()

@@ -319,9 +319,11 @@ int build_graph(Index* ix, int64_t n, const eps_build_params* params) {
   EPS_TRY(knn.reserve(static_cast<size_t>(n) * K * 8));
   if (n <= bp.exact_knn_below) {
     const int64_t qc = 8192;
+    ScanRequest r;  // the rows as queries
+    r.row_end = n; r.k = K; r.metric = ix->metric; r.skip_deleted = false;
     for (int64_t q0 = 0; q0 < n; q0 += qc) {
-      const int64_t nq = std::min(qc, n - q0);
-      EPS_TRY(brute_force_knn_rows(ix, q0, nq, n, K, knn.as<unsigned long long>() + q0 * K, &st));
+      r.queries = ix->d_vectors + q0 * ix->dim; r.nq = std::min(qc, n - q0); r.self_base = q0;
+      EPS_TRY(exact_topk(ix, r, knn.as<unsigned long long>() + q0 * K, &st));
     }
     EPS_CUDA(cudaStreamSynchronize(ix->stream));
   } else {
@@ -340,14 +342,9 @@ int build_graph(Index* ix, int64_t n, const eps_build_params* params) {
     column_sum_kernel<<<g, 128, 0, ix->stream>>>(ix->d_vectors, n, static_cast<int>(ix->dim), part.as<float>());
     centroid_kernel<<<static_cast<unsigned>((ix->dim + 127) / 128), 128, 0, ix->stream>>>(
         part.as<float>(), static_cast<int>(slices), static_cast<int>(ix->dim), 1.0f / static_cast<float>(n), cen.as<float>());
-    const int saved_metric = ix->metric;
-    const bool saved_del = ix->any_deleted;
-    ix->metric = EPS_METRIC_L2;
-    ix->any_deleted = false;
-    int rc = brute_force_topk(ix, cen.as<float>(), 1, 0, n, 1, nullptr, nullptr, false, top.as<unsigned long long>(), &st);
-    ix->metric = saved_metric;
-    ix->any_deleted = saved_del;
-    EPS_TRY(rc);
+    ScanRequest r;
+    r.queries = cen.as<float>(); r.nq = 1; r.row_end = n; r.k = 1; r.metric = EPS_METRIC_L2; r.skip_deleted = false;
+    EPS_TRY(exact_topk(ix, r, top.as<unsigned long long>(), &st));
     unsigned long long key;
     EPS_CUDA(cudaMemcpyAsync(&key, top.p, 8, cudaMemcpyDeviceToHost, ix->stream));
     EPS_CUDA(cudaStreamSynchronize(ix->stream));

@@ -194,41 +194,26 @@ int bind_program_columns(Index* ix, FilterProg* prog) {
   return check_like(ix, *prog);
 }
 
-// A search call's queries, dense or sparse: their graph search over [0, n_indexed) and the exact top-k of rows
-// [row_start, row_end).
+// A search call's queries, dense or sparse: their graph search over [0, n_indexed), and the exact scan's request
+// with the queries filled in.
 struct QueryBatch {
+  ScanRequest scan;
   virtual ~QueryBatch() = default;
   virtual int graph(Index* ix, int64_t L, unsigned long long* d_queue, eps_stats* st) const = 0;
-  virtual int scan(Index* ix, int64_t row_start, int64_t row_end, int64_t k, const FilterProg* d_prog,
-                   const FilterProg* h_prog, bool prefilter, unsigned long long* d_topk, eps_stats* st) const = 0;
 };
 
 struct DenseBatch : QueryBatch {
-  const float* d_queries;
-  int64_t nq;
-  DenseBatch(const float* q, int64_t n) : d_queries(q), nq(n) {}
+  DenseBatch(const float* q, int64_t nq) { scan.queries = q; scan.nq = nq; }
   int graph(Index* ix, int64_t L, unsigned long long* d_queue, eps_stats* st) const override {
-    return graph_search(ix, d_queries, nq, L, d_queue, st);
-  }
-  int scan(Index* ix, int64_t row_start, int64_t row_end, int64_t k, const FilterProg* d_prog, const FilterProg* h_prog,
-           bool prefilter, unsigned long long* d_topk, eps_stats* st) const override {
-    return brute_force_topk(ix, d_queries, nq, row_start, row_end, k, d_prog, h_prog, prefilter, d_topk, st);
+    return graph_search(ix, scan.queries, scan.nq, L, d_queue, st);
   }
 };
 
 struct SparseBatch : QueryBatch {
-  SparseDist dist;
-  SparseBatch(const SparseQueries& q, int64_t nq, int metric) {
-    dist.q = q;
-    dist.nq = nq;
-    dist.metric = metric;
-  }
+  const SparseDist& dist;  // the caller's: a copy of the batch still points at it
+  explicit SparseBatch(const SparseDist& d) : dist(d) { scan.dist = &d; scan.nq = d.nq; }
   int graph(Index* ix, int64_t L, unsigned long long* d_queue, eps_stats* st) const override {
     return sparse_graph_search(ix, dist.q, dist.nq, L, d_queue, st);
-  }
-  int scan(Index* ix, int64_t row_start, int64_t row_end, int64_t k, const FilterProg* d_prog, const FilterProg* h_prog,
-           bool prefilter, unsigned long long* d_topk, eps_stats* st) const override {
-    return scan_topk(ix, dist, dist.nq, row_start, row_end, k, d_prog, h_prog, prefilter, -1, d_topk, st);
   }
 };
 
@@ -256,6 +241,8 @@ static int run_search(Index* ix, const QueryBatch& qb, int64_t nq, int64_t limit
   eps_stats local;
   std::memset(&local, 0, sizeof(local));
   local.kernel_launches = like_launches;  // the LIKE pass
+  ScanRequest scan = qb.scan;
+  scan.metric = ix->metric; scan.d_prog = d_prog; scan.h_prog = &h_prog;
   if (stats) EPS_CUDA(cudaEventRecord(ix->ev[1], ix->stream));
   // BruteforceThreshold (hpp:28); a sparse index in EPS_SPARSE_SEARCH_SCAN always scans, whatever graph is installed
   const bool graph = !ix->prefilter && !ix->force_brute && n_indexed >= 512 &&
@@ -277,7 +264,8 @@ static int run_search(Index* ix, const QueryBatch& qb, int64_t nq, int64_t limit
       tail_k = std::min<int64_t>(std::min<int64_t>(limit, total - n_indexed), search_limit);
       if (tail_k > 8192) return fail(EPS_ERR_UNSUPPORTED, "more than 8192 tail results per query are not supported");
       EPS_TRY(ix->s_tail.reserve(static_cast<size_t>(nq) * tail_k * 8));
-      EPS_TRY(qb.scan(ix, n_indexed, total, tail_k, d_prog, &h_prog, false, ix->s_tail.as<unsigned long long>(), &local));
+      scan.row_start = n_indexed; scan.row_end = total; scan.k = tail_k;
+      EPS_TRY(exact_topk(ix, scan, ix->s_tail.as<unsigned long long>(), &local));
       d_tail = ix->s_tail.as<unsigned long long>();
     }
     EPS_TRY(finalize_graph(ix, ix->s_queue.as<unsigned long long>(), nq, L, search_limit, L, d_tail, tail_k, limit,
@@ -289,7 +277,8 @@ static int run_search(Index* ix, const QueryBatch& qb, int64_t nq, int64_t limit
     const int64_t k = std::max<int64_t>(1, std::min<int64_t>(cap, total));
     if (k > 8192) return fail(EPS_ERR_UNSUPPORTED, "more than 8192 results per query from the exact scan are not supported");
     EPS_TRY(ix->s_topk.reserve(static_cast<size_t>(nq) * k * 8));
-    EPS_TRY(qb.scan(ix, 0, total, k, d_prog, &h_prog, ix->prefilter, ix->s_topk.as<unsigned long long>(), &local));
+    scan.row_end = total; scan.k = k; scan.prefilter = ix->prefilter;
+    EPS_TRY(exact_topk(ix, scan, ix->s_topk.as<unsigned long long>(), &local));
     if (stats) EPS_CUDA(cudaEventRecord(ix->ev[2], ix->stream));
     EPS_TRY(finalize_keys(ix, ix->s_topk.as<unsigned long long>(), nq, k, limit, cap, d_ids, d_dists, d_counts));
   }
@@ -821,9 +810,10 @@ int eps_search_sparse_batch(eps_index* h, int64_t nq, const int64_t* q_offsets, 
   EPS_CUDA(cudaMemcpyAsync(d_q, qp.data(), ptr_bytes, cudaMemcpyHostToDevice, ix->stream));
   EPS_CUDA(cudaMemcpyAsync(d_q + nrm_off, qn.data(), static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, ix->stream));
   if (!qe.empty()) EPS_CUDA(cudaMemcpyAsync(d_q + el_off, qe.data(), qe.size() * 8, cudaMemcpyHostToDevice, ix->stream));
-  const eps::SparseQueries q{reinterpret_cast<const int64_t*>(d_q), reinterpret_cast<const uint2*>(d_q + el_off),
-                             reinterpret_cast<const float*>(d_q + nrm_off)};
-  return eps::search_to_host(ix, eps::SparseBatch(q, nq, ix->metric), nq, limit, filter, n_filter, out_ids, out_dists,
+  const eps::SparseDist dist(eps::SparseQueries{reinterpret_cast<const int64_t*>(d_q),
+                                                reinterpret_cast<const uint2*>(d_q + el_off),
+                                                reinterpret_cast<const float*>(d_q + nrm_off)}, nq);
+  return eps::search_to_host(ix, eps::SparseBatch(dist), nq, limit, filter, n_filter, out_ids, out_dists,
                              out_counts, stats);
 }
 

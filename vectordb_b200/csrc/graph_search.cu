@@ -870,8 +870,8 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   }
   const int64_t seed_ld = (L + 3) & ~3ll;
   EPS_TRY(ix->s_seed_dist.reserve(static_cast<size_t>(nq) * seed_ld * 4));
-  EPS_TRY(launch_distances(ix, ix->s_seed_rows.as<float>(), 0, L, d_queries, nq, ix->s_seed_dist.as<float>(), seed_ld,
-                           &launches));
+  EPS_TRY(launch_distances(ix, ix->metric, ix->s_seed_rows.as<float>(), 0, L, d_queries, nq, ix->s_seed_dist.as<float>(),
+                           seed_ld, &launches));
   GSArgs a;
   a.vectors = ix->d_vectors; a.offsets = ix->d_offsets; a.nbrs = ix->d_nbrs; a.ell = ix->d_ell;
   a.init_ids = ix->d_init_ids; a.seed_dist = ix->s_seed_dist.as<float>(); a.queries = d_queries;

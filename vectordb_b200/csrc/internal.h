@@ -147,17 +147,33 @@ struct Index : Table, Config {
 };
 
 // ---- brute_force.cu ------------------------------------------------------------------------
-// Exact top-k of rows [row_start,row_end) for nq device queries.  Writes per-query sorted keys
-// (make_key(dist,row)) to d_topk [nq x k] (kKeyInf padded).  Applies deleted bits and, if
-// prog != nullptr, the filter (prefilter=true evaluates it with distance 0).
-int brute_force_topk(Index* ix, const float* d_queries, int64_t nq, int64_t row_start, int64_t row_end, int64_t k,
-                     const FilterProg* d_prog, const FilterProg* h_prog, bool prefilter, unsigned long long* d_topk,
-                     eps_stats* stats);
+// Producer of the [nq x ldd] fp32 distance tile of rows [row_start, row_start + n) that the exact scan selects from,
+// in place of launch_distances (the sparse scan, sparse.cu).
+struct DistProducer {
+  virtual ~DistProducer() = default;
+  virtual int launch(Index* ix, int metric, int64_t row_start, int64_t n, float* D, int64_t ldd, uint64_t* launches) const = 0;
+};
+
+// One exact scan: everything it depends on besides the table itself.
+struct ScanRequest {
+  const float* queries = nullptr;      // dense queries [nq x dim] on the device, or
+  const DistProducer* dist = nullptr;  // a producer of the fp32 distance tile (never the tensor-core pass)
+  int64_t nq = 0, row_start = 0, row_end = 0, k = 0;
+  int metric = EPS_METRIC_L2;          // the field's; L2 for the build's navigation point (nsg.cpp)
+  const FilterProg* d_prog = nullptr;  // filter (device copy and host copy), or null
+  const FilterProg* h_prog = nullptr;
+  bool prefilter = false;              // evaluate the filter with distance 0
+  bool skip_deleted = true;            // false: the build indexes every row, deleted or not (ann_graph_segment.cpp:201)
+  int64_t self_base = -1;              // >= 0: row self_base + q is left out of query q's list (the build's kNN lists)
+};
+// Exact top-k of rows [row_start, row_end): per-query sorted keys (make_key(dist,row)) in d_topk [nq x k], kKeyInf
+// padded.
+int exact_topk(Index* ix, const ScanRequest& r, unsigned long long* d_topk, eps_stats* stats);
 
 // Distances of rows [row_start,row_start+n) of A_base to nq device queries: D[q*ldd + i] (row kernel for
 // nq <= 16, 128x128 tile kernel otherwise).
-int launch_distances(Index* ix, const float* A_base, int64_t row_start, int64_t n, const float* d_queries, int64_t nq,
-                     float* D, int64_t ldd, uint64_t* launches);
+int launch_distances(Index* ix, int metric, const float* A_base, int64_t row_start, int64_t n, const float* d_queries,
+                     int64_t nq, float* D, int64_t ldd, uint64_t* launches);
 
 // tc_dist.cu: wgmma TF32 / BF16 coarse distances (same contract as launch_distances, values carry ~1e-3 rel. error)
 bool tc_dist_usable(const Index* ix, int64_t nq);
@@ -169,24 +185,8 @@ struct TcFused {             // fused threshold selection in the epilogue (no di
   int64_t pass_base;
   int cand_cap;
 };
-int tc_launch_distances(Index* ix, int64_t row_start, int64_t n, const float* d_queries, int64_t nq, float* D, int64_t ldd,
-                        uint64_t* launches, const TcFused* fused = nullptr);
-
-// All-pairs variant used by the graph build: for queries = rows [q_start, q_start+nq) of the table.
-int brute_force_knn_rows(Index* ix, int64_t q_start, int64_t nq, int64_t n_rows, int64_t k,
-                         unsigned long long* d_topk, eps_stats* stats);
-
-// Producer of the [nq x ldd] fp32 distance tile of rows [row_start, row_start + n) that the exact scan selects from,
-// in place of launch_distances (the sparse scan, sparse.cu).
-struct DistProducer {
-  virtual ~DistProducer() = default;
-  virtual int launch(Index* ix, int64_t row_start, int64_t n, float* D, int64_t ldd, uint64_t* launches) const = 0;
-};
-// brute_force_topk with the distances of `dist` (nq queries): same pass bitmap, selection and key layout, never the
-// tensor-core pass.  self_base >= 0 excludes row self_base + q from query q's list (the build's kNN lists).
-int scan_topk(Index* ix, const DistProducer& dist, int64_t nq, int64_t row_start, int64_t row_end, int64_t k,
-              const FilterProg* d_prog, const FilterProg* h_prog, bool prefilter, int64_t self_base,
-              unsigned long long* d_topk, eps_stats* stats);
+int tc_launch_distances(Index* ix, int metric, int64_t row_start, int64_t n, const float* d_queries, int64_t nq, float* D,
+                        int64_t ldd, uint64_t* launches, const TcFused* fused = nullptr);
 
 // ---- sparse.cu -----------------------------------------------------------------------------
 // Queries of the sparse scan as a device CSR: ptr[q] .. ptr[q+1] index elems (absolute offsets), norm2[q] = the
@@ -199,8 +199,8 @@ struct SparseQueries {
 struct SparseDist : DistProducer {
   SparseQueries q;
   int64_t nq;
-  int metric;
-  int launch(Index* ix, int64_t row_start, int64_t n, float* D, int64_t ldd, uint64_t* launches) const override;
+  SparseDist(const SparseQueries& q_, int64_t nq_) : q(q_), nq(nq_) {}
+  int launch(Index* ix, int metric, int64_t row_start, int64_t n, float* D, int64_t ldd, uint64_t* launches) const override;
 };
 // Validate and pack n rows of a caller CSR (offsets[0..n], indices, values) into ptr (n+1 entries, starting at
 // ptr_base), elems and norm2.  Indices must be >= 0, < max_index and strictly increasing within a row.

@@ -457,25 +457,35 @@ bool tc_dist_usable(const Index* ix, int64_t nq) {
   return get_encode() != nullptr;
 }
 
+// Keeps a per-row mirror of the table current incrementally: room for the table's capacity, and convert(first, count)
+// for the rows appended since the last call; a buffer that moved is refilled from row 0.
+template <typename Convert>
+static int update_mirror(Index* ix, DevBuf* buf, size_t row_bytes, int64_t* rows, const void** ptr, uint64_t* launches,
+                         Convert convert) {
+  if (*rows >= ix->n_rows) return EPS_OK;
+  EPS_TRY(buf->reserve(static_cast<size_t>(std::max(ix->capacity, ix->n_rows)) * row_bytes));
+  if (buf->p != *ptr) { *rows = 0; *ptr = buf->p; }
+  EPS_TRY(convert(*rows, ix->n_rows - *rows));
+  *rows = ix->n_rows;
+  ++*launches;
+  return EPS_OK;
+}
+
 // Same contract as launch_distances() (D[q*ldd + i] for rows [row_start, row_start+n)), coarse values; with
 // `fused` the tile is filtered against the running thresholds in the epilogue instead of being written.
-int tc_launch_distances(Index* ix, int64_t row_start, int64_t n, const float* d_queries, int64_t nq, float* D,
+int tc_launch_distances(Index* ix, int metric, int64_t row_start, int64_t n, const float* d_queries, int64_t nq, float* D,
                         int64_t ldd, uint64_t* launches, const TcFused* fused) {
   const int dim = static_cast<int>(ix->dim);
   const bool bf16 = ix->coarse_mode == 2;
   // |x|^2 of every row and the table's largest (every metric: the guard scales its error sample by the norm ratio)
-  if (ix->xnorm_rows < ix->n_rows) {  // row norms for rows appended since the last call
-    EPS_TRY(ix->s_xnorm.reserve(static_cast<size_t>(ix->capacity > ix->n_rows ? ix->capacity : ix->n_rows) * 4));
+  EPS_TRY(update_mirror(ix, &ix->s_xnorm, 4, &ix->xnorm_rows, &ix->xnorm_ptr, launches, [&](int64_t first, int64_t cnt) {
     EPS_TRY(ix->s_xnorm_max.reserve(4));
-    if (ix->s_xnorm.p != ix->xnorm_ptr) { ix->xnorm_rows = 0; ix->xnorm_ptr = ix->s_xnorm.p; }
-    if (ix->xnorm_rows == 0) EPS_CUDA(cudaMemsetAsync(ix->s_xnorm_max.p, 0, 4, ix->stream));
-    const int64_t cnt = ix->n_rows - ix->xnorm_rows;
+    if (first == 0) EPS_CUDA(cudaMemsetAsync(ix->s_xnorm_max.p, 0, 4, ix->stream));
     row_norm_kernel<<<static_cast<unsigned>((cnt * 32 + 255) / 256), 256, 0, ix->stream>>>(
-        ix->d_vectors, ix->xnorm_rows, cnt, dim, ix->s_xnorm.as<float>(), ix->s_xnorm_max.as<unsigned>());
-    ix->xnorm_rows = ix->n_rows;
-    ++*launches;
-  }
-  if (ix->metric == EPS_METRIC_L2) {
+        ix->d_vectors, first, cnt, dim, ix->s_xnorm.as<float>(), ix->s_xnorm_max.as<unsigned>());
+    return EPS_OK;
+  }));
+  if (metric == EPS_METRIC_L2) {
     EPS_TRY(ix->s_qnorm.reserve(static_cast<size_t>(nq) * 4));
     row_norm_kernel<<<static_cast<unsigned>((nq * 32 + 255) / 256), 256, 0, ix->stream>>>(d_queries, 0, nq, dim,
                                                                                          ix->s_qnorm.as<float>());
@@ -484,16 +494,13 @@ int tc_launch_distances(Index* ix, int64_t row_start, int64_t n, const float* d_
   const void* a_base = ix->d_vectors;
   const void* b_base = d_queries;
   if (bf16) {
-    // bf16 mirror of the table (coarse pass only; the re-score reads the fp32 rows), kept current incrementally
-    if (ix->bf16_rows < ix->n_rows) {
-      EPS_TRY(ix->s_bf16.reserve(static_cast<size_t>(ix->capacity > ix->n_rows ? ix->capacity : ix->n_rows) * dim * 2));
-      if (ix->s_bf16.p != ix->bf16_ptr) { ix->bf16_rows = 0; ix->bf16_ptr = ix->s_bf16.p; }
-      const int64_t cnt = (ix->n_rows - ix->bf16_rows) * dim;
-      to_bf16_kernel<<<static_cast<unsigned>((cnt / 4 + 256) / 256), 256, 0, ix->stream>>>(
-          ix->d_vectors + ix->bf16_rows * dim, cnt, ix->s_bf16.as<unsigned short>() + ix->bf16_rows * dim);
-      ix->bf16_rows = ix->n_rows;
-      ++*launches;
-    }
+    // bf16 mirror of the table (coarse pass only; the re-score reads the fp32 rows)
+    auto to_bf16 = [&](int64_t first, int64_t cnt) {
+      to_bf16_kernel<<<static_cast<unsigned>((cnt * dim / 4 + 256) / 256), 256, 0, ix->stream>>>(
+          ix->d_vectors + first * dim, cnt * dim, ix->s_bf16.as<unsigned short>() + first * dim);
+      return EPS_OK;
+    };
+    EPS_TRY(update_mirror(ix, &ix->s_bf16, static_cast<size_t>(dim) * 2, &ix->bf16_rows, &ix->bf16_ptr, launches, to_bf16));
     EPS_TRY(ix->s_qbf16.reserve(static_cast<size_t>(nq) * dim * 2));
     const int64_t cnt = nq * dim;
     to_bf16_kernel<<<static_cast<unsigned>((cnt / 4 + 256) / 256), 256, 0, ix->stream>>>(d_queries, cnt, ix->s_qbf16.as<unsigned short>());
@@ -504,11 +511,10 @@ int tc_launch_distances(Index* ix, int64_t row_start, int64_t n, const float* d_
   CUtensorMap tmA, tmB;
   EPS_TRY(make_map(&tmA, a_base, ix->n_rows, dim, kTcBM, bf16));
   EPS_TRY(make_map(&tmB, b_base, nq, dim, kTcBN, bf16));
-  TcArgs a;
+  TcArgs a = {};
   a.row_start = row_start; a.n = n; a.nq = nq; a.ldd = ldd;
-  a.xnorm = ix->s_xnorm.as<float>(); a.qnorm = ix->s_qnorm.as<float>(); a.D = D; a.dim = dim; a.metric = ix->metric;
+  a.xnorm = ix->s_xnorm.as<float>(); a.qnorm = ix->s_qnorm.as<float>(); a.D = D; a.dim = dim; a.metric = metric;
   a.kb_elems = bf16 ? 64 : 32;
-  a.thr = nullptr; a.cand = nullptr; a.cand_cnt = nullptr; a.pass = nullptr; a.pass_base = 0; a.cand_cap = 0;
   if (fused) {
     a.D = nullptr;
     a.thr = fused->thr; a.cand = fused->cand; a.cand_cnt = fused->cand_cnt; a.pass = fused->pass;
@@ -516,15 +522,10 @@ int tc_launch_distances(Index* ix, int64_t row_start, int64_t n, const float* d_
   }
   a.n_row_tiles = static_cast<int>((n + kTcBM - 1) / kTcBM);
   a.n_q_tiles = static_cast<int>((nq + kTcBN - 1) / kTcBN);
-  static bool attr_set = false;
-  if (!attr_set) {
-    EPS_CUDA(cudaFuncSetAttribute(tc_dist_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmem));
-    EPS_CUDA(cudaFuncSetAttribute(tc_dist_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmem));
-    attr_set = true;
-  }
-  const int grid = std::min(a.n_row_tiles, ix->num_sms);
-  if (bf16) tc_dist_kernel<true><<<grid, kTcThreads, kTcSmem, ix->stream>>>(tmA, tmB, a);
-  else tc_dist_kernel<false><<<grid, kTcThreads, kTcSmem, ix->stream>>>(tmA, tmB, a);
+  // per call: the attribute belongs to the current device, and one process may hold indexes on several
+  const auto kernel = bf16 ? tc_dist_kernel<true> : tc_dist_kernel<false>;
+  EPS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmem));
+  kernel<<<std::min(a.n_row_tiles, ix->num_sms), kTcThreads, kTcSmem, ix->stream>>>(tmA, tmB, a);
   EPS_CUDA(cudaGetLastError());
   ++*launches;
   return EPS_OK;

@@ -510,7 +510,7 @@ static int pass_bitmap(Index* ix, const ScanRequest& r, uint32_t** d_pass, uint6
   EPS_TRY(ix->s_pass.reserve(static_cast<size_t>(words) * 4));
   *d_pass = ix->s_pass.as<uint32_t>();
   pass_bitmap_kernel<<<static_cast<unsigned>((words + 127) / 128), 128, 0, ix->stream>>>(
-      deleted ? ix->d_deleted : nullptr, ix->deleted_bytes, filter ? r.d_prog : nullptr, ix->d_attrs, ix->attr_stride,
+      deleted ? ix->d_deleted.as<const uint8_t>() : nullptr, ix->deleted_bytes, filter ? r.d_prog : nullptr, ix->d_attrs, ix->attr_stride,
       r.row_start, n, *d_pass);
   ++*launches;
   return EPS_OK;

@@ -212,8 +212,8 @@ static int prune_pass(Index* ix, int64_t n, const unsigned long long* d_knn, int
 
 int install_csr(Index* ix, int64_t n, const int64_t* off, const int32_t* nb, int64_t e, int64_t nav) {
   free_graph(ix);
-  EPS_CUDA(cudaMalloc(&ix->d_offsets, (static_cast<size_t>(n) + 1) * 8));
-  EPS_CUDA(cudaMalloc(&ix->d_nbrs, std::max<size_t>(static_cast<size_t>(e), 1) * 4));
+  EPS_TRY(ix->d_offsets.reserve((static_cast<size_t>(n) + 1) * 8));
+  EPS_TRY(ix->d_nbrs.reserve(std::max<size_t>(static_cast<size_t>(e), 1) * 4));
   EPS_CUDA(cudaMemcpyAsync(ix->d_offsets, off, (static_cast<size_t>(n) + 1) * 8, cudaMemcpyHostToDevice, ix->stream));
   if (e > 0) EPS_CUDA(cudaMemcpyAsync(ix->d_nbrs, nb, static_cast<size_t>(e) * 4, cudaMemcpyHostToDevice, ix->stream));
   EPS_CUDA(cudaStreamSynchronize(ix->stream));

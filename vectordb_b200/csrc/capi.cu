@@ -4,6 +4,7 @@
 #include <cstdio>
 #include <algorithm>
 #include <cstring>
+#include <memory>
 #include <mutex>
 
 #include "internal.h"
@@ -17,22 +18,52 @@ int fail(int code, const std::string& msg) {
   return code;
 }
 
-int DevBuf::reserve(size_t bytes) {
+int Mem::reserve(size_t bytes) {
   if (bytes <= cap && p) return EPS_OK;
-  if (p) { cudaFree(p); p = nullptr; cap = 0; }
-  size_t want = bytes < 256 ? 256 : bytes;
-  cudaError_t e = cudaMalloc(&p, want);
-  if (e != cudaSuccess) {
-    p = nullptr;
-    return fail(EPS_ERR_OOM, std::string("cudaMalloc(") + std::to_string(want) + "): " + cudaGetErrorString(e));
-  }
-  cap = want;
+  release();
+  void* q = nullptr;
+  const cudaError_t e = host ? cudaHostAlloc(&q, bytes, cudaHostAllocDefault) : cudaMalloc(&q, bytes);
+  if (e != cudaSuccess)
+    return fail(EPS_ERR_OOM, std::string(host ? "cudaHostAlloc(" : "cudaMalloc(") + std::to_string(bytes) + "): " +
+                                 cudaGetErrorString(e));
+  p = q;
+  cap = bytes;
+  owns = true;
+  ++gen;
   return EPS_OK;
 }
-void DevBuf::release() {
-  if (p) cudaFree(p);
+
+int Mem::grow(size_t bytes, size_t keep, cudaStream_t s) {
+  if (bytes <= cap && p) return EPS_OK;
+  Mem fresh;
+  EPS_TRY(fresh.reserve(bytes));
+  if (p && keep > 0) {
+    EPS_CUDA(cudaMemcpyAsync(fresh.p, p, keep, cudaMemcpyDeviceToDevice, s));
+    EPS_CUDA(cudaStreamSynchronize(s));
+  }
+  release();
+  std::swap(p, fresh.p);
+  std::swap(cap, fresh.cap);
+  std::swap(owns, fresh.owns);
+  ++gen;
+  return EPS_OK;
+}
+
+void Mem::release() {
+  if (p && owns) {
+    if (host) cudaFreeHost(p);
+    else cudaFree(p);
+  }
   p = nullptr;
   cap = 0;
+  owns = false;
+}
+
+void Mem::alias(void* q, size_t bytes) {
+  release();
+  p = q;
+  cap = bytes;
+  ++gen;
 }
 
 int check_device(int device) {
@@ -148,16 +179,12 @@ __global__ void narrow_ids_kernel(const int64_t* __restrict__ in, int64_t n, int
 }
 
 void free_graph(Index* ix) {
-  if (ix->d_offsets) cudaFree(ix->d_offsets);
-  if (ix->d_nbrs) cudaFree(ix->d_nbrs);
-  if (ix->d_init_ids) cudaFree(ix->d_init_ids);
-  if (ix->d_ell) cudaFree(ix->d_ell);
-  ix->d_ell = nullptr;
+  ix->d_offsets.release();
+  ix->d_nbrs.release();
+  ix->d_init_ids.release();
+  ix->d_ell.release();
   free_sketch(ix);
   ix->seed_rows_L = 0;
-  ix->d_offsets = nullptr;
-  ix->d_nbrs = nullptr;
-  ix->d_init_ids = nullptr;
   ix->init_L = 0;
   ix->n_indexed = 0;
   ix->n_edges = 0;
@@ -317,20 +344,14 @@ static int search_to_host(Index* ix, const QueryBatch& qb, int64_t nq, int64_t l
   const size_t n_ids = static_cast<size_t>(nq) * limit;
   const size_t off_cnt = n_ids * 8, off_dist = off_cnt + static_cast<size_t>(nq) * 8, total = off_dist + n_ids * 4;
   EPS_TRY(ix->s_out_ids.reserve(total));
-  if (ix->h_out_cap < total) {
-    if (ix->h_out) cudaFreeHost(ix->h_out);
-    ix->h_out = nullptr;
-    ix->h_out_cap = 0;
-    EPS_CUDA(cudaHostAlloc(&ix->h_out, total, cudaHostAllocDefault));
-    ix->h_out_cap = total;
-  }
+  EPS_TRY(ix->h_out.reserve(total));
   unsigned char* d_blk = ix->s_out_ids.as<unsigned char>();
   EPS_TRY(run_search(ix, qb, nq, limit, filter, n_filter, reinterpret_cast<int64_t*>(d_blk),
                      reinterpret_cast<float*>(d_blk + off_dist), reinterpret_cast<int64_t*>(d_blk + off_cnt), stats));
-  EPS_CUDA(cudaMemcpyAsync(ix->h_out, d_blk, total, cudaMemcpyDeviceToHost, ix->stream));
+  EPS_CUDA(cudaMemcpyAsync(ix->h_out.p, d_blk, total, cudaMemcpyDeviceToHost, ix->stream));
   if (stats) EPS_CUDA(cudaEventRecord(ix->ev[3], ix->stream));
   EPS_CUDA(cudaStreamSynchronize(ix->stream));
-  const unsigned char* hb = static_cast<const unsigned char*>(ix->h_out);
+  const unsigned char* hb = ix->h_out.as<const unsigned char>();
   std::memcpy(out_ids, hb, n_ids * 8);
   std::memcpy(out_counts, hb + off_cnt, static_cast<size_t>(nq) * 8);
   const float* hd = reinterpret_cast<const float*>(hb + off_dist);
@@ -367,7 +388,7 @@ int eps_index_create(eps_index** out, int metric, int64_t dim, const float* host
   if (metric != EPS_METRIC_L2 && metric != EPS_METRIC_COSINE && metric != EPS_METRIC_IP)
     metric = EPS_METRIC_L2;  // GetDistFunc default branch (db/index/index.cpp:19-20)
   EPS_TRY(eps::check_device(device));
-  Index* ix = new Index();
+  std::unique_ptr<Index> ix(new Index());  // deleted on the error paths with its device current
   ix->device = device;
   ix->metric = metric;
   ix->dim = dim;
@@ -376,19 +397,11 @@ int eps_index_create(eps_index** out, int metric, int64_t dim, const float* host
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) ix->num_sms = prop.multiProcessorCount;
   cudaError_t e = cudaStreamCreateWithFlags(&ix->stream, cudaStreamNonBlocking);
-  if (e != cudaSuccess) { delete ix; return eps::fail(EPS_ERR_CUDA, cudaGetErrorString(e)); }
+  if (e != cudaSuccess) return eps::fail(EPS_ERR_CUDA, cudaGetErrorString(e));
   for (auto& ev : ix->ev) cudaEventCreate(&ev);
-  if (capacity_rows > 0 && host_vectors) {
-    e = cudaMalloc(&ix->d_vectors, static_cast<size_t>(capacity_rows) * dim * 4);
-    if (e != cudaSuccess) {
-      cudaStreamDestroy(ix->stream);
-      delete ix;
-      return eps::fail(EPS_ERR_OOM, std::string("vector table: ") + cudaGetErrorString(e));
-    }
-    ix->owns_vectors = true;
-  }
+  if (capacity_rows > 0 && host_vectors) EPS_TRY(ix->d_vectors.reserve(static_cast<size_t>(capacity_rows) * dim * 4));
   ix->vec4 = (dim % 4 == 0);
-  *out = reinterpret_cast<eps_index*>(ix);
+  *out = reinterpret_cast<eps_index*>(ix.release());
   return EPS_OK;
 }
 
@@ -405,14 +418,16 @@ int eps_index_create_sparse(eps_index** out, int metric, int64_t dim, int64_t ca
   ix->sparse = true;
   ix->capacity = capacity_rows;
   const int64_t rows = std::max<int64_t>(capacity_rows, 1);
-  cudaError_t e = cudaMalloc(&ix->d_sp_ptr, static_cast<size_t>(rows + 1) * 8);
-  if (e == cudaSuccess) e = cudaMalloc(&ix->d_sp_norm2, static_cast<size_t>(rows) * 4);
-  if (e == cudaSuccess) e = cudaMemset(ix->d_sp_ptr, 0, 8);
-  if (e != cudaSuccess) {
+  auto row_table = [&]() -> int {
+    EPS_TRY(ix->d_sp_ptr.reserve(static_cast<size_t>(rows + 1) * 8));
+    EPS_TRY(ix->d_sp_norm2.reserve(static_cast<size_t>(rows) * 4));
+    EPS_CUDA(cudaMemset(ix->d_sp_ptr, 0, 8));
+    return EPS_OK;
+  };
+  if (const int rc = row_table(); rc != EPS_OK) {
     eps_index_destroy(h);
-    return eps::fail(EPS_ERR_OOM, std::string("sparse row table: ") + cudaGetErrorString(e));
+    return rc;
   }
-  ix->sp_row_cap = rows;
   *out = h;
   return EPS_OK;
 }
@@ -422,37 +437,18 @@ void eps_index_destroy(eps_index* h) {
   Index* ix = reinterpret_cast<Index*>(h);
   cudaSetDevice(ix->device);
   cudaStreamSynchronize(ix->stream);
-  if (ix->view_of) {  // a view owns its seed set, stream and scratch only
-    if (ix->d_init_ids) cudaFree(ix->d_init_ids);
-    Index* base = ix->view_of;
+  if (Index* base = ix->view_of) {
     --base->n_views;
     base->views.erase(std::remove(base->views.begin(), base->views.end(), ix), base->views.end());
-  } else if (ix->detached_view) {
-    if (ix->d_init_ids) cudaFree(ix->d_init_ids);  // its base went first: nothing shared is left to release
-  } else {
-    for (Index* v : ix->views) {  // base destroyed before its views: they become empty indexes instead of dangling
-      cudaStreamSynchronize(v->stream);
-      v->view_of = nullptr; v->detached_view = true;
-      const int64_t nav = v->nav;  // eps_index_get_graph still reports it
-      static_cast<eps::Table&>(*v) = eps::Table();
-      v->nav = nav;
-    }
-    ix->views.clear();
-    eps::free_graph(ix);
-    if (ix->owns_vectors && ix->d_vectors) cudaFree(ix->d_vectors);
-    if (ix->d_deleted) cudaFree(ix->d_deleted);
-    if (ix->d_attrs) cudaFree(ix->d_attrs);
-    for (auto& sc : ix->str_cols) if (sc.d_codes) cudaFree(sc.d_codes);
-    eps::free_dict(&ix->dict);
-    if (ix->d_sp_ptr) cudaFree(ix->d_sp_ptr);
-    if (ix->d_sp_elems) cudaFree(ix->d_sp_elems);
-    if (ix->d_sp_norm2) cudaFree(ix->d_sp_norm2);
   }
-  if (ix->h_out) cudaFreeHost(ix->h_out);
-  if (ix->d_screened) cudaFree(ix->d_screened);
-  for (auto& ev : ix->ev) if (ev) cudaEventDestroy(ev);
-  cudaStreamDestroy(ix->stream);
-  delete ix;  // the scratch DevBufs release themselves
+  for (Index* v : ix->views) {  // base destroyed before its views: they become empty indexes instead of dangling
+    cudaStreamSynchronize(v->stream);
+    v->view_of = nullptr; v->detached_view = true;
+    const int64_t nav = v->nav;  // eps_index_get_graph still reports it
+    static_cast<eps::Table&>(*v) = eps::Table();
+    v->nav = nav;
+  }
+  delete ix;
 }
 
 // A read-only view of an index: the same device table, graph and segment mirrors, its own stream and scratch.
@@ -495,7 +491,7 @@ int eps_index_sync_rows(eps_index* h, int64_t n_rows_now) {
   EPS_TRY(eps::check_device(ix->device));
   EPS_TRY(eps::dense_only(ix));
   EPS_TRY(check_mutable(ix));
-  if (!ix->owns_vectors) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "index has no host vector table to mirror");
+  if (!ix->d_vectors.owns) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "index has no host vector table to mirror");
   if (n_rows_now < ix->n_rows || n_rows_now > ix->capacity)
     return eps::fail(EPS_ERR_INVALID_ARGUMENT, "n_rows_now outside [mirrored rows, capacity]");
   if (n_rows_now > ix->n_rows) {
@@ -515,9 +511,7 @@ int eps_index_adopt_device_rows(eps_index* h, const float* d_vectors, int64_t n_
   EPS_TRY(eps::check_device(ix->device));
   EPS_TRY(check_mutable(ix));
   if (n_rows < 0 || n_rows >= (1ll << 31)) return eps::fail(EPS_ERR_UNSUPPORTED, "row count must be in [0, 2^31): keys carry 31-bit ids");
-  if (ix->owns_vectors && ix->d_vectors) cudaFree(ix->d_vectors);
-  ix->owns_vectors = false;
-  ix->d_vectors = const_cast<float*>(d_vectors);
+  ix->d_vectors.alias(const_cast<float*>(d_vectors), static_cast<size_t>(n_rows) * ix->dim * 4);
   // state derived from the previous table: gathered seed rows always, the graph itself if it no longer fits
   ix->seed_rows_L = 0;
   eps::free_sketch(ix);  // computed from the rows this call replaces
@@ -547,8 +541,8 @@ int eps_index_set_graph(eps_index* h, int64_t n_indexed, const int64_t* offsets,
   for (int64_t i = 0; i < n_indexed; ++i)
     if (offsets[i + 1] < offsets[i]) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "offset table is not monotonic");
   if (e > 0 && !nbrs) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null neighbor list");
-  EPS_CUDA(cudaMalloc(&ix->d_offsets, (static_cast<size_t>(n_indexed) + 1) * 8));
-  EPS_CUDA(cudaMalloc(&ix->d_nbrs, static_cast<size_t>(e > 0 ? e : 1) * 4));
+  EPS_TRY(ix->d_offsets.reserve((static_cast<size_t>(n_indexed) + 1) * 8));
+  EPS_TRY(ix->d_nbrs.reserve(static_cast<size_t>(e > 0 ? e : 1) * 4));
   EPS_CUDA(cudaMemcpyAsync(ix->d_offsets, offsets, (static_cast<size_t>(n_indexed) + 1) * 8, cudaMemcpyHostToDevice, ix->stream));
   // neighbour ids: int64 in the reference CSR, int32 on the device — narrowed and range-checked by a kernel over
   // 64M-edge chunks (a host loop over 4e8 edges costs seconds)
@@ -616,7 +610,7 @@ int eps_index_set_deleted(eps_index* h, const uint8_t* bitset, int64_t nbytes) {
   EPS_TRY(check_mutable(ix));
   if (!bitset || nbytes <= 0) { ix->any_deleted = false; ix->deleted_bytes = 0; ix->h_deleted.clear(); return EPS_OK; }
   int64_t lo = 0, hi = nbytes;  // dirty span [lo, hi)
-  const bool same_geometry = ix->d_deleted && static_cast<int64_t>(ix->h_deleted.size()) == nbytes && nbytes <= ix->deleted_cap;
+  const bool same_geometry = ix->d_deleted && static_cast<int64_t>(ix->h_deleted.size()) == nbytes && nbytes <= ix->d_deleted.count();
   if (same_geometry) {
     const uint8_t* old = ix->h_deleted.data();
     int64_t w = 0;
@@ -628,19 +622,18 @@ int eps_index_set_deleted(eps_index* h, const uint8_t* bitset, int64_t nbytes) {
     hi = nbytes;
     while (hi > lo && old[hi - 1] == bitset[hi - 1]) --hi;
   } else {
-    if (nbytes > ix->deleted_cap) {
-      if (ix->d_deleted) cudaFree(ix->d_deleted);
-      ix->d_deleted = nullptr;
-      // room for the whole table so that growth of record_number_ never reallocates
-      const int64_t cap = std::max<int64_t>(nbytes, (ix->capacity + 7) / 8 + 8);
-      EPS_CUDA(cudaMalloc(&ix->d_deleted, static_cast<size_t>(cap)));
-      ix->deleted_cap = cap;
-    }
-    ix->h_deleted.assign(static_cast<size_t>(nbytes), 0);
+    // room for the whole table so that growth of record_number_ never reallocates; the old bitmap is freed only
+    // once the new one is allocated, so a failure leaves the mirror as it was
+    if (nbytes > ix->d_deleted.count())
+      EPS_TRY(ix->d_deleted.grow(static_cast<size_t>(std::max<int64_t>(nbytes, (ix->capacity + 7) / 8 + 8)), 0, ix->stream));
+    // nothing is known to be on the device until the whole bitset is
+    ix->h_deleted.clear();
+    ix->deleted_bytes = 0;
     ix->any_deleted = false;
   }
   EPS_CUDA(cudaMemcpyAsync(ix->d_deleted + lo, bitset + lo, static_cast<size_t>(hi - lo), cudaMemcpyHostToDevice, ix->stream));
   EPS_CUDA(cudaStreamSynchronize(ix->stream));
+  ix->h_deleted.resize(static_cast<size_t>(nbytes));
   std::memcpy(ix->h_deleted.data() + lo, bitset + lo, static_cast<size_t>(hi - lo));
   ix->deleted_bytes = nbytes;
   if (!ix->any_deleted) {
@@ -659,18 +652,17 @@ int eps_index_set_attrs(eps_index* h, const char* table, int64_t stride, int64_t
   EPS_TRY(eps::check_device(ix->device));
   EPS_TRY(check_mutable(ix));
   if (!table || stride <= 0 || n_rows <= 0) {
-    if (ix->d_attrs) { cudaFree(ix->d_attrs); ix->d_attrs = nullptr; }
-    ix->attr_stride = stride; ix->attr_rows = 0; ix->attr_cap_rows = 0; ix->attr_src = nullptr;
+    ix->d_attrs.release();
+    ix->attr_stride = stride; ix->attr_rows = 0; ix->attr_src = nullptr;
     return EPS_OK;
   }
   int64_t first = 0;
-  if (ix->d_attrs && ix->attr_src == table && ix->attr_stride == stride && n_rows >= ix->attr_rows && n_rows <= ix->attr_cap_rows) {
+  if (ix->d_attrs && ix->attr_src == table && ix->attr_stride == stride && n_rows >= ix->attr_rows &&
+      n_rows <= static_cast<int64_t>(ix->d_attrs.cap) / stride) {
     first = ix->attr_rows;  // append
   } else {
-    if (ix->d_attrs) { cudaFree(ix->d_attrs); ix->d_attrs = nullptr; }
-    const int64_t cap = std::max<int64_t>(n_rows, ix->capacity);
-    EPS_CUDA(cudaMalloc(&ix->d_attrs, static_cast<size_t>(stride) * cap));
-    ix->attr_cap_rows = cap;
+    ix->d_attrs.release();
+    EPS_TRY(ix->d_attrs.reserve(static_cast<size_t>(stride) * std::max<int64_t>(n_rows, ix->capacity)));
   }
   ix->attr_stride = stride;
   ix->attr_src = table;
@@ -695,18 +687,9 @@ int eps_index_set_string_codes(eps_index* h, int column, int64_t first_row, cons
   eps::StrCol& sc = ix->str_cols[column];
   if (first_row > sc.rows) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "string codes must be appended without gaps");
   const int64_t need = first_row + count;
-  if (need > sc.cap) {
-    const int64_t cap = std::max<int64_t>(need, std::max<int64_t>(ix->capacity, 2 * sc.cap));
-    int32_t* fresh = nullptr;
-    EPS_CUDA(cudaMalloc(&fresh, static_cast<size_t>(cap) * 4));
-    if (sc.d_codes && sc.rows > 0) {
-      cudaError_t e = cudaMemcpyAsync(fresh, sc.d_codes, static_cast<size_t>(sc.rows) * 4, cudaMemcpyDeviceToDevice, ix->stream);
-      if (e == cudaSuccess) e = cudaStreamSynchronize(ix->stream);
-      if (e != cudaSuccess) { cudaFree(fresh); return eps::fail(EPS_ERR_CUDA, cudaGetErrorString(e)); }
-    }
-    if (sc.d_codes) cudaFree(sc.d_codes);
-    sc.d_codes = fresh;
-    sc.cap = cap;
+  if (need > sc.d_codes.count()) {
+    const int64_t cap = std::max<int64_t>(need, std::max<int64_t>(ix->capacity, 2 * sc.d_codes.count()));
+    EPS_TRY(sc.d_codes.grow(static_cast<size_t>(cap) * 4, static_cast<size_t>(sc.rows) * 4, ix->stream));
   }
   if (count > 0) {
     EPS_CUDA(cudaMemcpyAsync(sc.d_codes + first_row, codes, static_cast<size_t>(count) * 4, cudaMemcpyHostToDevice, ix->stream));
@@ -830,36 +813,30 @@ int eps_normalize(int device, float* host_vectors, int64_t nq, int64_t dim) {
   if (nq <= 0) return EPS_OK;
   if (!host_vectors || dim < 1) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null vectors / bad dim");
   const size_t bytes = static_cast<size_t>(nq) * dim * 4;
-  float* d = nullptr;
-  EPS_CUDA(cudaMalloc(&d, bytes));
-  cudaError_t e = cudaMemcpy(d, host_vectors, bytes, cudaMemcpyHostToDevice);
-  int rc = EPS_OK;
-  if (e == cudaSuccess) rc = eps::normalize_rows_device(nullptr, d, nq, dim);
-  if (e == cudaSuccess && rc == EPS_OK) e = cudaMemcpy(host_vectors, d, bytes, cudaMemcpyDeviceToHost);
-  cudaFree(d);
-  if (e != cudaSuccess) return eps::fail(EPS_ERR_CUDA, cudaGetErrorString(e));
-  return rc;
+  eps::Mem d;
+  EPS_TRY(d.reserve(bytes));
+  EPS_CUDA(cudaMemcpy(d.p, host_vectors, bytes, cudaMemcpyHostToDevice));
+  EPS_TRY(eps::normalize_rows_device(nullptr, d.as<float>(), nq, dim));
+  EPS_CUDA(cudaMemcpy(host_vectors, d.p, bytes, cudaMemcpyDeviceToHost));
+  return EPS_OK;
 }
 
 int eps_pair_distances(int device, int metric, const float* a, const float* b, int64_t n, int64_t dim, float* out) {
   EPS_TRY(eps::check_device(device));
   if (n <= 0) return EPS_OK;
   if (!a || !b || !out || dim < 1) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null argument / bad dim");
-  float *da = nullptr, *db = nullptr, *dout = nullptr;
   const size_t bytes = static_cast<size_t>(n) * dim * 4;
-  cudaError_t e = cudaMalloc(&da, bytes);
-  if (e == cudaSuccess) e = cudaMalloc(&db, bytes);
-  if (e == cudaSuccess) e = cudaMalloc(&dout, static_cast<size_t>(n) * 4);
-  if (e == cudaSuccess) e = cudaMemcpy(da, a, bytes, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(db, b, bytes, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) {
-    eps::pair_distance_kernel<<<static_cast<unsigned>((n * 32 + 127) / 128), 128>>>(metric, dim % 4 == 0 ? 1 : 0, da, db, n,
-                                                                                   static_cast<int>(dim), dout);
-    e = cudaDeviceSynchronize();
-  }
-  if (e == cudaSuccess) e = cudaMemcpy(out, dout, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost);
-  cudaFree(da); cudaFree(db); cudaFree(dout);
-  if (e != cudaSuccess) return eps::fail(EPS_ERR_CUDA, cudaGetErrorString(e));
+  eps::Mem da, db, dout;
+  EPS_TRY(da.reserve(bytes));
+  EPS_TRY(db.reserve(bytes));
+  EPS_TRY(dout.reserve(static_cast<size_t>(n) * 4));
+  EPS_CUDA(cudaMemcpy(da.p, a, bytes, cudaMemcpyHostToDevice));
+  EPS_CUDA(cudaMemcpy(db.p, b, bytes, cudaMemcpyHostToDevice));
+  eps::pair_distance_kernel<<<static_cast<unsigned>((n * 32 + 127) / 128), 128>>>(metric, dim % 4 == 0 ? 1 : 0, da.as<float>(),
+                                                                                 db.as<float>(), n, static_cast<int>(dim),
+                                                                                 dout.as<float>());
+  EPS_CUDA(cudaDeviceSynchronize());
+  EPS_CUDA(cudaMemcpy(out, dout.p, static_cast<size_t>(n) * 4, cudaMemcpyDeviceToHost));
   return EPS_OK;
 }
 

@@ -165,7 +165,7 @@ int finalize_graph(Index* ix, unsigned long long* d_queue, int64_t nq, int64_t L
   const int blocks = static_cast<int>((nq * 32 + threads - 1) / threads);
   finalize_graph_kernel<<<blocks, threads, 0, ix->stream>>>(
       d_queue, static_cast<int>(nq), static_cast<int>(L), static_cast<int>(search_limit), static_cast<int>(cand_num),
-      d_tail, static_cast<int>(tail_k), static_cast<int>(limit), ix->any_deleted ? ix->d_deleted : nullptr,
+      d_tail, static_cast<int>(tail_k), static_cast<int>(limit), ix->any_deleted ? ix->d_deleted.as<const uint8_t>() : nullptr,
       ix->deleted_bytes, has_prog ? d_prog : nullptr, ix->d_attrs, ix->attr_stride, d_ids, d_dists, d_counts);
   EPS_CUDA(cudaGetLastError());
   return EPS_OK;

@@ -778,8 +778,8 @@ int prepare_init_ids(Index* ix, int64_t L) {
     sel[v] = true;
     ids.push_back(static_cast<int32_t>(v));
   }
-  if (ix->d_init_ids) { cudaFree(ix->d_init_ids); ix->d_init_ids = nullptr; }
-  EPS_CUDA(cudaMalloc(&ix->d_init_ids, static_cast<size_t>(L) * 4));
+  ix->d_init_ids.release();
+  EPS_TRY(ix->d_init_ids.reserve(static_cast<size_t>(L) * 4));
   EPS_CUDA(cudaMemcpyAsync(ix->d_init_ids, ids.data(), static_cast<size_t>(L) * 4, cudaMemcpyHostToDevice, ix->stream));
   EPS_CUDA(cudaStreamSynchronize(ix->stream));
   ix->init_L = L;
@@ -797,7 +797,7 @@ static int ring_slots_for(const Index* ix, int slot_bytes) {
 
 int ensure_ell(Index* ix, uint64_t* launches) {
   if (ix->d_ell || !ix->d_offsets) return EPS_OK;
-  EPS_CUDA(cudaMalloc(&ix->d_ell, static_cast<size_t>(ix->n_indexed) * kEll * 4));
+  EPS_TRY(ix->d_ell.reserve(static_cast<size_t>(ix->n_indexed) * kEll * 4));
   const int64_t tot = ix->n_indexed * kEll;
   csr_to_ell_kernel<<<static_cast<unsigned>((tot + 255) / 256), 256, 0, ix->stream>>>(ix->d_offsets, ix->d_nbrs, ix->n_indexed, ix->d_ell);
   EPS_CUDA(cudaGetLastError());
@@ -887,7 +887,7 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   a.sk = nullptr; a.qsk = nullptr; a.n_sk = 0; a.sk_g = 0.f; a.sk_scale = 0.f; a.n_screened = nullptr;
   if (screen) {
     if (!ix->d_screened) {
-      EPS_CUDA(cudaMalloc(&ix->d_screened, 8));
+      EPS_TRY(ix->d_screened.reserve(8));
       EPS_CUDA(cudaMemsetAsync(ix->d_screened, 0, 8, ix->stream));
     }
     EPS_TRY(ix->s_qsk.reserve(static_cast<size_t>(nq) * (kSketch + 1) * 4));
@@ -941,13 +941,11 @@ int prepare_visited(Index* ix, int slots, int64_t L, VisitedSets* v) {
     EPS_TRY(ix->s_visited.reserve(static_cast<size_t>(slots) * words * 4));
     ix->visited_slots = slots;
   }
-  // bitmaps must start clean; the kernel leaves them clean.  (Re)zero when the geometry changed.
-  // (a re-grown buffer may come back at the old address: the capacity is part of the geometry)
-  if (ix->vis_clean_ptr != ix->s_visited.p || ix->vis_clean_words != words || ix->vis_clean_cap != ix->s_visited.cap) {
+  // bitmaps must start clean; the kernel leaves them clean.  (Re)zero when the buffer or the geometry changed.
+  if (ix->visited_gen != ix->s_visited.gen || ix->visited_words != words) {
     EPS_CUDA(cudaMemsetAsync(ix->s_visited.p, 0, ix->s_visited.cap, ix->stream));
-    ix->vis_clean_ptr = ix->s_visited.p;
-    ix->vis_clean_words = words;
-    ix->vis_clean_cap = ix->s_visited.cap;
+    ix->visited_gen = ix->s_visited.gen;
+    ix->visited_words = words;
   }
   // Visited hash sets: 16 entries per queue slot, so that the ~10 L ids a query visits load its table about 2/3 (a
   // query that needs more moves to its bitmap), and at most 16384 entries = 64 KB per slot: the tables of the 528
@@ -955,10 +953,9 @@ int prepare_visited(Index* ix, int slots, int64_t L, VisitedSets* v) {
   // touched, so the whole buffer is all-ones between launches whatever the table size; fill it when it is (re)allocated.
   const int vset_cap = std::min(16384, std::max(1024, next_pow2(16 * static_cast<int>(L))));
   EPS_TRY(ix->s_vset.reserve(static_cast<size_t>(slots) * vset_cap * 4));
-  if (ix->vset_clean_ptr != ix->s_vset.p || ix->vset_clean_cap != ix->s_vset.cap) {
+  if (ix->vset_gen != ix->s_vset.gen) {
     EPS_CUDA(cudaMemsetAsync(ix->s_vset.p, 0xff, ix->s_vset.cap, ix->stream));
-    ix->vset_clean_ptr = ix->s_vset.p;
-    ix->vset_clean_cap = ix->s_vset.cap;
+    ix->vset_gen = ix->s_vset.gen;
   }
   // fresh ids of the running query in FIFO order: the migration to the bitmap and the bitmap reset read them
   constexpr int kVlogCap = 32768;

@@ -10,24 +10,56 @@
 
 namespace eps {
 
-// Device buffer that grows on demand (never shrinks); owned by an index / a call context.
-struct DevBuf {
+// Device memory (pinned host memory when `host`) with its capacity in bytes.  This is the only code that allocates or
+// frees; an alias refers to memory the object does not own and never frees it.
+struct Mem {
   void* p = nullptr;
   size_t cap = 0;
-  DevBuf() = default;
-  DevBuf(const DevBuf&) = delete;
-  DevBuf& operator=(const DevBuf&) = delete;
-  ~DevBuf() { release(); }  // error paths (EPS_TRY / EPS_CUDA early returns) must not leak device memory
+  bool owns = false;
+  bool host = false;
+  uint64_t gen = 0;  // bumped whenever p takes new memory: contents filled under an older generation are gone
+  Mem() = default;
+  Mem(const Mem&) = delete;
+  Mem& operator=(const Mem&) = delete;
+  ~Mem() { release(); }  // error paths (EPS_TRY / EPS_CUDA early returns) must not leak device memory
+  // Room for `bytes`; when that needs an allocation, the old memory is freed first and exactly `bytes` are allocated.
   int reserve(size_t bytes);
+  // Room for `bytes`, keeping the first `keep` (a device-to-device copy on s); the old memory is freed last, so a
+  // failure leaves the buffer as it was.
+  int grow(size_t bytes, size_t keep, cudaStream_t s);
   void release();
+  void alias(void* q, size_t bytes);
   template <typename T>
-  T* as() { return static_cast<T*>(p); }
+  T* as() const { return static_cast<T*>(p); }
+};
+
+// Scratch buffer that grows on demand (never shrinks, at least 256 bytes); owned by an index / a call context.
+struct DevBuf : Mem {
+  int reserve(size_t bytes) { return Mem::reserve(bytes < 256 ? 256 : bytes); }
+};
+
+// Pinned host buffer.
+struct HostBuf : Mem {
+  HostBuf() { host = true; }
+};
+
+// Device array of T.  A copy is a non-owning alias of the same memory: a view assigned its base's Table frees nothing.
+template <typename T>
+struct DevArray : Mem {
+  DevArray() = default;
+  DevArray(const DevArray& o) : Mem() { alias(o.p, o.cap); }
+  DevArray& operator=(const DevArray& o) {
+    if (this != &o) alias(o.p, o.cap);
+    return *this;
+  }
+  operator T*() const { return static_cast<T*>(p); }
+  int64_t count() const { return static_cast<int64_t>(cap / sizeof(T)); }  // elements there is room for
 };
 
 // Device mirror of one string column as dictionary codes (filter.cuh).
 struct StrCol {
-  int32_t* d_codes = nullptr;
-  int64_t rows = 0, cap = 0;
+  DevArray<int32_t> d_codes;
+  int64_t rows = 0;
   bool any_negative = false;  // some mirrored code is < 0 (a LIKE cannot read the column then)
   int32_t max_code = -1;      // largest mirrored code
 };
@@ -35,42 +67,40 @@ struct StrCol {
 // Device mirror of the caller's string dictionary (like.cu): code c is bytes[off[c] .. off[c+1]).  Append-only,
 // grown like StrCol; a view shares its base's.
 struct StrDict {
-  int64_t* d_off = nullptr;  // [n + 1], d_off[0] = 0
-  char* d_bytes = nullptr;
-  int64_t n = 0, cap = 0;               // codes mirrored / room for codes
-  int64_t bytes = 0, byte_cap = 0;
+  DevArray<int64_t> d_off;  // [n + 1], d_off[0] = 0
+  DevArray<char> d_bytes;
+  int64_t n = 0;            // codes mirrored
+  int64_t bytes = 0;
 };
 
 // Device data a base owns and its views alias; only the base frees it.
 struct Table {
   int64_t capacity = 0;
-  float* d_vectors = nullptr;   // [capacity x dim] (owned unless adopted)
+  DevArray<float> d_vectors;    // [capacity x dim] (an alias of the caller's rows once adopted)
   int64_t n_rows = 0;           // rows mirrored so far (record_number_ snapshot)
   bool vec4 = false;            // dim % 4 == 0 and 16-B aligned base
 
   // sparse column (eps_index_create_sparse): rows are a CSR of {uint32 index, float value} elements
-  int64_t* d_sp_ptr = nullptr;  // [sp_row_cap + 1] element offsets of the rows
-  uint2* d_sp_elems = nullptr;  // [sp_elem_cap] {index, value bits}, indices strictly increasing within a row
-  float* d_sp_norm2 = nullptr;  // [sp_row_cap] sequential fp32 sum of squares of each row (cosine)
-  int64_t sp_nnz = 0, sp_elem_cap = 0, sp_row_cap = 0;
+  DevArray<int64_t> d_sp_ptr;   // [rows + 1] element offsets of the rows
+  DevArray<uint2> d_sp_elems;   // {index, value bits}, indices strictly increasing within a row
+  DevArray<float> d_sp_norm2;   // [rows] sequential fp32 sum of squares of each row (cosine); its room is the row room
+  int64_t sp_nnz = 0;
 
   // graph (ANNGraphSegment mirror)
   int64_t n_indexed = 0;
   int64_t n_edges = 0;
   int64_t nav = 0;
-  int64_t* d_offsets = nullptr;  // [n_indexed + 1]
-  int32_t* d_nbrs = nullptr;     // [n_edges]
-  int32_t* d_ell = nullptr;      // fixed-stride adjacency [n_indexed x 64] (-1 padded), built lazily
+  DevArray<int64_t> d_offsets;  // [n_indexed + 1]
+  DevArray<int32_t> d_nbrs;     // [n_edges]
+  DevArray<int32_t> d_ell;      // fixed-stride adjacency [n_indexed x 64] (-1 padded), built lazily
 
   // segment mirrors
-  uint8_t* d_deleted = nullptr;
+  DevArray<uint8_t> d_deleted;
   int64_t deleted_bytes = 0;
-  int64_t deleted_cap = 0;
   bool any_deleted = false;
-  char* d_attrs = nullptr;
+  DevArray<char> d_attrs;
   int64_t attr_stride = 0;
   int64_t attr_rows = 0;
-  int64_t attr_cap_rows = 0;
   StrCol str_cols[kMaxStringCols];
   StrDict dict;
 
@@ -81,8 +111,8 @@ struct Table {
   float sk_g = 0.f;              // 1 - gamma_{m+2}, rounded down
   float sk_scale = 0.f;          // (1 - 2 (dim + 2) 2^-24) / (1 + eps), rounded down
   double sk_eps = 0.0;           // sigma_max(P~)^2 <= 1 + sk_eps
-  float* d_sk_basis = nullptr;   // [dim x sk_m] fp32 basis P~ (transposed), then [dim] mean
-  float* d_sk = nullptr;         // [n_indexed x sk_m] row sketches, then [n_indexed] their error bounds (null: screen off)
+  DevArray<float> d_sk_basis;    // [dim x sk_m] fp32 basis P~ (transposed), then [dim] mean
+  DevArray<float> d_sk;          // [n_indexed x sk_m] row sketches, then [n_indexed] their error bounds (null: screen off)
 };
 
 // Executor and tuning parameters: a view starts with its base's and sets its own afterwards.
@@ -100,6 +130,7 @@ struct Config {
   int graph_screen = EPS_GRAPH_SCREEN_AUTO;
 };
 
+// Deleted with its device current (eps_index_destroy): it frees what it owns, never its base's Table.
 struct Index : Table, Config {
   int device = 0;
   int metric = EPS_METRIC_L2;
@@ -107,7 +138,6 @@ struct Index : Table, Config {
   bool sparse = false;
   int num_sms = 132;
   const float* host_vectors = nullptr;
-  bool owns_vectors = false;
   Index* view_of = nullptr;     // read-only view (eps_index_create_view): its Table belongs to this index
   int n_views = 0;              // live views of this index; mutating entry points refuse while > 0
   std::vector<Index*> views;    // the live views (detached when the base is destroyed first)
@@ -115,35 +145,36 @@ struct Index : Table, Config {
   std::vector<uint8_t> h_deleted;  // host shadow of the uploaded deleted bitset (dirty-span detection)
   const char* attr_src = nullptr;  // host table the attribute mirror was filled from (append detection)
 
-  int32_t* d_init_ids = nullptr; // seed set for init_L
+  DevArray<int32_t> d_init_ids;  // seed set for init_L
   int64_t init_L = 0;
   int64_t seed_rows_L = 0;       // L for which s_seed_rows holds the gathered seed rows
 
   cudaStream_t stream = nullptr;
   cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+  ~Index() {
+    for (auto& e : ev) if (e) cudaEventDestroy(e);
+    if (stream) cudaStreamDestroy(stream);
+  }
 
   // scratch
   DevBuf s_queries, s_dist, s_topk, s_topk2, s_pass, s_filter, s_vset, s_visited, s_vlog, s_queue, s_tail, s_out_ids, s_out_dists,
       s_out_counts, s_stats, s_misc, s_seed_rows, s_seed_dist, s_xnorm, s_qnorm, s_coarse, s_thr, s_cand, s_cand_cnt, s_bf16, s_qbf16, s_flags,
       s_sparse_q, s_xnorm_max, s_like, s_like_jobs;
-  int64_t bf16_rows = 0;
-  const void* bf16_ptr = nullptr;
+  int64_t bf16_rows = 0;         // rows converted into s_bf16 while it had generation bf16_gen
+  uint64_t bf16_gen = 0;
   int64_t xnorm_rows = 0;        // rows whose |x|^2 is current in s_xnorm; s_xnorm_max holds the largest (float bits)
-  const void* xnorm_ptr = nullptr;
+  uint64_t xnorm_gen = 0;
   int64_t visited_slots = 0;
-  const void* vis_clean_ptr = nullptr;  // geometry for which the visited bitmaps are known to be zero
-  int64_t vis_clean_words = 0;
-  size_t vis_clean_cap = 0;
-  const void* vset_clean_ptr = nullptr;  // visited hash-set buffer known to be all-ones (empty), and its capacity
-  size_t vset_clean_cap = 0;
+  uint64_t visited_gen = 0;      // s_visited generation and bitmap words for which the bitmaps are known to be zero
+  int64_t visited_words = 0;
+  uint64_t vset_gen = 0;         // s_vset generation known to be all-ones (empty)
   bool graph_counters_pending = false;
   int64_t prof_nq = 0;           // developer build (EPS_GS_PROFILE): queries of the last graph-search launch
   DevBuf s_prof_qtimes;          // developer build: [prof_nq x 4] per-query timeline of the last dense launch
   bool prof_timeline = false;    // developer build: s_prof_qtimes belongs to the last launch
   DevBuf s_qsk;                  // [nq x sk_m] query sketches, then [nq] their error bounds
-  unsigned long long* d_screened = nullptr;  // device count of the fresh neighbours the screen dropped on this handle
-  void* h_out = nullptr;         // pinned host mirror of the packed result block (eps_search_batch)
-  size_t h_out_cap = 0;
+  DevArray<unsigned long long> d_screened;  // device count of the fresh neighbours the screen dropped on this handle
+  HostBuf h_out;                 // pinned host mirror of the packed result block (eps_search_batch)
 };
 
 // ---- brute_force.cu ------------------------------------------------------------------------
@@ -303,7 +334,6 @@ struct ConnRepair {
 // ---- like.cu -------------------------------------------------------------------------------
 // Append codes [first_code, first_code + count) to the dictionary mirror (eps_index_append_string_dictionary).
 int dict_append(Index* ix, int64_t first_code, int64_t count, const int64_t* offsets, const char* bytes);
-void free_dict(StrDict* d);
 // Validation of the LIKE nodes of a lowered program (constant codes and the columns they read); bind_program_columns
 // calls it, so every failure comes before any launch.
 int check_like(const Index* ix, const FilterProg& prog);

@@ -93,30 +93,6 @@ __global__ void like_kernel(const LikeJob* __restrict__ jobs, int n_jobs, int64_
   if ((threadIdx.x & 31) == 0 && item < jb.n_items) jb.out[item >> 5] = w;
 }
 
-void free_dict(StrDict* d) {
-  if (d->d_off) cudaFree(d->d_off);
-  if (d->d_bytes) cudaFree(d->d_bytes);
-  *d = StrDict();
-}
-
-// Grow a device array to hold `need` elements of `elem` bytes, keeping its first `keep` elements.
-static int grow(Index* ix, void** p, int64_t* cap, int64_t need, int64_t keep, size_t elem) {
-  if (need <= *cap && *p) return EPS_OK;
-  const int64_t want = std::max<int64_t>(need, std::max<int64_t>(2 * *cap, 256));
-  void* fresh = nullptr;
-  cudaError_t e = cudaMalloc(&fresh, static_cast<size_t>(want) * elem);
-  if (e != cudaSuccess) return fail(EPS_ERR_OOM, std::string("string dictionary: ") + cudaGetErrorString(e));
-  if (*p && keep > 0) {
-    e = cudaMemcpyAsync(fresh, *p, static_cast<size_t>(keep) * elem, cudaMemcpyDeviceToDevice, ix->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ix->stream);
-    if (e != cudaSuccess) { cudaFree(fresh); return fail(EPS_ERR_CUDA, cudaGetErrorString(e)); }
-  }
-  if (*p) cudaFree(*p);
-  *p = fresh;
-  *cap = want;
-  return EPS_OK;
-}
-
 int dict_append(Index* ix, int64_t first_code, int64_t count, const int64_t* offsets, const char* bytes) {
   StrDict& d = ix->dict;
   if (count < 0) return fail(EPS_ERR_INVALID_ARGUMENT, "negative string count");
@@ -130,8 +106,15 @@ int dict_append(Index* ix, int64_t first_code, int64_t count, const int64_t* off
   if (offsets[0] < 0) return fail(EPS_ERR_INVALID_ARGUMENT, "negative string offset");
   if (d.n + count > INT32_MAX) return fail(EPS_ERR_UNSUPPORTED, "more than 2^31 - 1 dictionary codes (codes are int32)");
   const int64_t span = offsets[count] - offsets[0];
-  EPS_TRY(grow(ix, reinterpret_cast<void**>(&d.d_off), &d.cap, d.n + count + 1, d.n + 1, 8));
-  EPS_TRY(grow(ix, reinterpret_cast<void**>(&d.d_bytes), &d.byte_cap, d.bytes + span, d.bytes, 1));
+  // room for `need` elements, keeping the first `keep`: doubling, at least 256 (allocated on the first append)
+  auto room = [&](Mem& m, size_t elem, int64_t need, int64_t keep) {
+    const int64_t cap = static_cast<int64_t>(m.cap / elem);
+    if (need <= cap && m.p) return EPS_OK;
+    const int64_t want = std::max<int64_t>(need, std::max<int64_t>(2 * cap, 256));
+    return m.grow(static_cast<size_t>(want) * elem, static_cast<size_t>(keep) * elem, ix->stream);
+  };
+  EPS_TRY(room(d.d_off, 8, d.n + count + 1, d.n + 1));
+  EPS_TRY(room(d.d_bytes, 1, d.bytes + span, d.bytes));
   std::vector<int64_t> off(static_cast<size_t>(count) + (d.n == 0 ? 1 : 0));
   size_t k = 0;
   if (d.n == 0) off[k++] = 0;
@@ -216,7 +199,7 @@ int bind_like(Index* ix, FilterProg* progs, int n, uint64_t* launches) {
   constexpr int kThreads = 256;
   like_kernel<<<static_cast<unsigned>((items + kThreads - 1) / kThreads), kThreads, 0, ix->stream>>>(
       ix->s_like_jobs.as<LikeJob>(), static_cast<int>(jobs.size()), items, ix->dict.d_off,
-      reinterpret_cast<const uint8_t*>(ix->dict.d_bytes));
+      ix->dict.d_bytes.as<const uint8_t>());
   EPS_CUDA(cudaGetLastError());
   if (launches) *launches += 1;
   return EPS_OK;

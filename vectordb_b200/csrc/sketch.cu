@@ -153,15 +153,9 @@ float round_down(double x) {
 
 }  // namespace
 
-void free_sketch_rows(Index* ix) {
-  if (ix->d_sk) cudaFree(ix->d_sk);
-  ix->d_sk = nullptr;
-}
-
 void free_sketch(Index* ix) {
-  free_sketch_rows(ix);
-  if (ix->d_sk_basis) cudaFree(ix->d_sk_basis);
-  ix->d_sk_basis = nullptr;
+  ix->d_sk.release();
+  ix->d_sk_basis.release();
   ix->sk_m = 0;
   ix->sk_share = -1.0;
 }
@@ -173,7 +167,7 @@ int sketch_rows(Index* ix, const float* d_x, int64_t n, float* d_sk, float* d_ex
   const size_t smem = static_cast<size_t>(kSkRows) * (dim + 1) * 4;
   EPS_CUDA(cudaFuncSetAttribute(sketch_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   sketch_rows_kernel<<<static_cast<unsigned>((n + kSkRows - 1) / kSkRows), 256, smem, ix->stream>>>(
-      d_x, n, dim, reinterpret_cast<const float4*>(ix->d_sk_basis), ix->d_sk_basis + static_cast<int64_t>(dim) * kSketch,
+      d_x, n, dim, ix->d_sk_basis.as<const float4>(), ix->d_sk_basis + static_cast<int64_t>(dim) * kSketch,
       sm * gam * std::sqrt(1.0 + ix->sk_eps), sm * dim * 0x1.0p-149, d_sk, d_ex);
   EPS_CUDA(cudaGetLastError());
   return EPS_OK;
@@ -210,7 +204,7 @@ int compute_sketch(Index* ix) {
     for (int j = 0; j < m; ++j)
       for (int k = 0; k < dim; ++k) up[static_cast<size_t>(k) * m + j] = basis[static_cast<size_t>(j) * dim + k];
     for (int k = 0; k < dim; ++k) up[static_cast<size_t>(dim) * m + k] = mean[k];
-    EPS_CUDA(cudaMalloc(&ix->d_sk_basis, up.size() * 4));
+    EPS_TRY(ix->d_sk_basis.reserve(up.size() * 4));
     EPS_CUDA(cudaMemcpyAsync(ix->d_sk_basis, up.data(), up.size() * 4, cudaMemcpyHostToDevice, ix->stream));
     EPS_CUDA(cudaStreamSynchronize(ix->stream));
     ix->sk_m = m;
@@ -220,11 +214,11 @@ int compute_sketch(Index* ix) {
     ix->sk_scale = round_down((1.0 - 2.0 * (dim + 2) * u) / (1.0 + eps));
   }
   const bool want = ix->graph_screen == EPS_GRAPH_SCREEN_ON || ix->sk_share >= kScreenShare;
-  if (!want) free_sketch_rows(ix);
+  if (!want) ix->d_sk.release();
 
   if (want && !ix->d_sk) {
     const int64_t n = ix->n_indexed;
-    EPS_CUDA(cudaMalloc(&ix->d_sk, static_cast<size_t>(n) * (m + 1) * 4));  // [n x m] sketches, then [n] bounds
+    EPS_TRY(ix->d_sk.reserve(static_cast<size_t>(n) * (m + 1) * 4));  // [n x m] sketches, then [n] bounds
     EPS_TRY(sketch_rows(ix, ix->d_vectors, n, ix->d_sk, ix->d_sk + n * m));
     EPS_CUDA(cudaStreamSynchronize(ix->stream));
   }
@@ -236,7 +230,7 @@ int compute_sketch(Index* ix) {
 void ensure_sketch(Index* ix) {
   if (ix->metric != EPS_METRIC_L2 || ix->graph_screen == EPS_GRAPH_SCREEN_OFF || ix->dim < 128 || ix->n_indexed < 1 ||
       !ix->d_vectors) {
-    free_sketch_rows(ix);
+    ix->d_sk.release();
     return;
   }
   // the screen only saves time: when it cannot be set up (out of device memory), the search runs without it

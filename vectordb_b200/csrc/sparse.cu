@@ -190,19 +190,6 @@ int pack_sparse(int64_t n, const int64_t* offsets, const int64_t* indices, const
   return EPS_OK;
 }
 
-static int grow(void** p, size_t used_bytes, size_t want_bytes, cudaStream_t s) {
-  void* fresh = nullptr;
-  EPS_CUDA(cudaMalloc(&fresh, want_bytes));
-  if (*p && used_bytes > 0) {
-    cudaError_t e = cudaMemcpyAsync(fresh, *p, used_bytes, cudaMemcpyDeviceToDevice, s);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) { cudaFree(fresh); return fail(EPS_ERR_CUDA, cudaGetErrorString(e)); }
-  }
-  if (*p) cudaFree(*p);
-  *p = fresh;
-  return EPS_OK;
-}
-
 int sparse_append(Index* ix, int64_t first_row, int64_t n_rows, const int64_t* offsets, const int64_t* indices,
                   const float* values) {
   if (first_row != ix->n_rows) return fail(EPS_ERR_INVALID_ARGUMENT, "rows must be appended after the mirrored ones (first_row != rows)");
@@ -214,17 +201,15 @@ int sparse_append(Index* ix, int64_t first_row, int64_t n_rows, const int64_t* o
   std::vector<float> nrm;
   EPS_TRY(pack_sparse(n_rows, offsets, indices, values, ix->dim, ix->sp_nnz, &ptr, &el, &nrm));
   const int64_t rows = ix->n_rows + n_rows, nnz = ix->sp_nnz + static_cast<int64_t>(el.size());
-  if (rows > ix->sp_row_cap) {
-    const int64_t cap = std::max<int64_t>(rows, 2 * ix->sp_row_cap);
-    EPS_TRY(grow(reinterpret_cast<void**>(&ix->d_sp_ptr), static_cast<size_t>(ix->n_rows + 1) * 8, static_cast<size_t>(cap + 1) * 8, ix->stream));
-    EPS_TRY(grow(reinterpret_cast<void**>(&ix->d_sp_norm2), static_cast<size_t>(ix->n_rows) * 4, static_cast<size_t>(cap) * 4, ix->stream));
-    ix->sp_row_cap = cap;
+  if (rows > ix->d_sp_norm2.count()) {
+    const int64_t cap = std::max<int64_t>(rows, 2 * ix->d_sp_norm2.count());
+    EPS_TRY(ix->d_sp_ptr.grow(static_cast<size_t>(cap + 1) * 8, static_cast<size_t>(ix->n_rows + 1) * 8, ix->stream));
+    EPS_TRY(ix->d_sp_norm2.grow(static_cast<size_t>(cap) * 4, static_cast<size_t>(ix->n_rows) * 4, ix->stream));
     ix->capacity = std::max(ix->capacity, cap);
   }
-  if (nnz > ix->sp_elem_cap) {
-    const int64_t cap = std::max<int64_t>(nnz, 2 * ix->sp_elem_cap);
-    EPS_TRY(grow(reinterpret_cast<void**>(&ix->d_sp_elems), static_cast<size_t>(ix->sp_nnz) * 8, static_cast<size_t>(std::max<int64_t>(cap, 1)) * 8, ix->stream));
-    ix->sp_elem_cap = std::max<int64_t>(cap, 1);
+  if (nnz > ix->d_sp_elems.count()) {
+    const int64_t cap = std::max<int64_t>(nnz, 2 * ix->d_sp_elems.count());
+    EPS_TRY(ix->d_sp_elems.grow(static_cast<size_t>(cap) * 8, static_cast<size_t>(ix->sp_nnz) * 8, ix->stream));
   }
   // ptr[0] (= the current nnz) is already on the device
   EPS_CUDA(cudaMemcpyAsync(ix->d_sp_ptr + ix->n_rows + 1, ptr.data() + 1, static_cast<size_t>(n_rows) * 8, cudaMemcpyHostToDevice, ix->stream));

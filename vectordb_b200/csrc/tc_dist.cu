@@ -453,18 +453,18 @@ bool tc_dist_usable(const Index* ix, int64_t nq) {
   if (nq < 64 || nq > 1024) return false;            // per-query constants live in a 4 KB shared-memory table
   const int align = ix->coarse_mode == 2 ? 8 : 4;    // TMA: 16-byte row pitch
   if (ix->dim % align != 0 || ix->dim < 32) return false;
-  if ((reinterpret_cast<uintptr_t>(ix->d_vectors) & 15) != 0) return false;
+  if ((reinterpret_cast<uintptr_t>(ix->d_vectors.p) & 15) != 0) return false;
   return get_encode() != nullptr;
 }
 
 // Keeps a per-row mirror of the table current incrementally: room for the table's capacity, and convert(first, count)
-// for the rows appended since the last call; a buffer that moved is refilled from row 0.
+// for the rows appended since the last call; a buffer reallocated since (a new generation) is refilled from row 0.
 template <typename Convert>
-static int update_mirror(Index* ix, DevBuf* buf, size_t row_bytes, int64_t* rows, const void** ptr, uint64_t* launches,
+static int update_mirror(Index* ix, DevBuf* buf, size_t row_bytes, int64_t* rows, uint64_t* gen, uint64_t* launches,
                          Convert convert) {
   if (*rows >= ix->n_rows) return EPS_OK;
   EPS_TRY(buf->reserve(static_cast<size_t>(std::max(ix->capacity, ix->n_rows)) * row_bytes));
-  if (buf->p != *ptr) { *rows = 0; *ptr = buf->p; }
+  if (buf->gen != *gen) { *rows = 0; *gen = buf->gen; }
   EPS_TRY(convert(*rows, ix->n_rows - *rows));
   *rows = ix->n_rows;
   ++*launches;
@@ -478,7 +478,7 @@ int tc_launch_distances(Index* ix, int metric, int64_t row_start, int64_t n, con
   const int dim = static_cast<int>(ix->dim);
   const bool bf16 = ix->coarse_mode == 2;
   // |x|^2 of every row and the table's largest (every metric: the guard scales its error sample by the norm ratio)
-  EPS_TRY(update_mirror(ix, &ix->s_xnorm, 4, &ix->xnorm_rows, &ix->xnorm_ptr, launches, [&](int64_t first, int64_t cnt) {
+  EPS_TRY(update_mirror(ix, &ix->s_xnorm, 4, &ix->xnorm_rows, &ix->xnorm_gen, launches, [&](int64_t first, int64_t cnt) {
     EPS_TRY(ix->s_xnorm_max.reserve(4));
     if (first == 0) EPS_CUDA(cudaMemsetAsync(ix->s_xnorm_max.p, 0, 4, ix->stream));
     row_norm_kernel<<<static_cast<unsigned>((cnt * 32 + 255) / 256), 256, 0, ix->stream>>>(
@@ -500,7 +500,7 @@ int tc_launch_distances(Index* ix, int metric, int64_t row_start, int64_t n, con
           ix->d_vectors + first * dim, cnt * dim, ix->s_bf16.as<unsigned short>() + first * dim);
       return EPS_OK;
     };
-    EPS_TRY(update_mirror(ix, &ix->s_bf16, static_cast<size_t>(dim) * 2, &ix->bf16_rows, &ix->bf16_ptr, launches, to_bf16));
+    EPS_TRY(update_mirror(ix, &ix->s_bf16, static_cast<size_t>(dim) * 2, &ix->bf16_rows, &ix->bf16_gen, launches, to_bf16));
     EPS_TRY(ix->s_qbf16.reserve(static_cast<size_t>(nq) * dim * 2));
     const int64_t cnt = nq * dim;
     to_bf16_kernel<<<static_cast<unsigned>((cnt / 4 + 256) / 256), 256, 0, ix->stream>>>(d_queries, cnt, ix->s_qbf16.as<unsigned short>());

@@ -147,6 +147,29 @@ EPS_API int eps_index_set_graph(eps_index* ix, int64_t n_indexed, const int64_t*
  * [0, n): kNN graph (db/index/knn) + NSG-style refinement (db/index/nsg), installed into the index. */
 EPS_API int eps_index_build(eps_index* ix, int64_t n, const eps_build_params* params);
 
+/* Link rows [n_indexed, n) of the mirrored table into the installed graph, so that afterwards n_indexed = n and searches
+ * no longer scan those rows as the tail (vec_search_executor.cpp:885-900) — without the full rebuild that
+ * TableMVP::Rebuild runs (db/table_mvp.cpp:94-203).  params as for eps_index_build (NULL = defaults); knn_k,
+ * out_degree, candidate_pool, search_length, min_degree, alpha and seed are read.
+ * Works on any installed dense graph: one built by eps_index_build or installed by eps_index_set_graph (a graph the
+ * reference built included).  n == n_indexed does nothing and returns EPS_OK (the graph stays bitwise identical).
+ * Errors: no graph installed, n < n_indexed, n above the mirrored rows, a view, an index with live views, or a sparse
+ * index: EPS_ERR_INVALID_ARGUMENT; n >= 2^31: EPS_ERR_UNSUPPORTED; a failed argument check changes nothing.
+ * Like the build, every row is indexed, deleted or not (ann_graph_segment.cpp:201).  The new rows are linked in
+ * chunks of 65 536: each new row's candidates are the pool of a graph search over the graph as the previous chunks left
+ * it (field metric, width 4, L = 128) merged with its exact kNN among the rows of its chunk (field metric), selected
+ * with the build's L2 SelectEdge rule, and offered as reverse edges to their targets.  A new row gets at most
+ * min(out_degree, 64) selected edges.  An old row changes only by being re-selected over its row and the new rows
+ * offered to it, by having offered rows appended while it fits out_degree, or by repair edges appended at its end (the
+ * build's repair: a vertex the navigation point does not reach is attached to the nearest reached vertex its own search
+ * finds); a row already wider than out_degree (e.g. the navigation point with its component entries) is left as it is.  The navigation point does not change.  On return every row of [0, n) is
+ * reachable from it.  The same table, graph, n and params give the same graph on every run.
+ * The graph screen's basis, mean and share are kept, not re-sampled from the grown table; stored row sketches are
+ * extended to the new rows.  The call's own searches are not screened and do not count in n_screened.
+ * Device memory the call adds: a second CSR while the graph is spliced, [n x 64] int32 adjacency rows (which the search
+ * keeps anyway), O(n) int32 / int64 arrays and per-chunk buffers (DESIGN.md §K4, B4). */
+EPS_API int eps_index_extend_graph(eps_index* ix, int64_t n, const eps_build_params* params);
+
 /* Copy the installed graph out as the reference's int64 CSR (the payload of ann_graph_<field>.bin,
  * db/ann_graph_segment.cpp:171-184).  Pass NULL buffers to query sizes. */
 EPS_API int eps_index_get_graph(eps_index* ix, int64_t* n_indexed, int64_t* n_edges, int64_t* offset_table,
@@ -321,7 +344,7 @@ EPS_API int eps_pair_distances(int device, int metric, const float* a, const flo
  * These calls work on a sparse index as on a dense one: eps_index_set_deleted, eps_index_set_attrs,
  * eps_index_set_string_codes, eps_index_config, eps_index_create_view (the view shares the CSR), eps_index_build,
  * eps_index_get_graph, eps_index_rows, eps_facet_batch.  The dense-only calls (sync_rows, adopt_device_rows,
- * device_rows, set_graph, set_coarse, set_search_width, set_graph_tuning, eps_search_batch*,
+ * device_rows, set_graph, extend_graph, set_coarse, set_search_width, set_graph_tuning, eps_search_batch*,
  * eps_search_batch_sharded) fail with EPS_ERR_INVALID_ARGUMENT (device_rows returns NULL).
  * --------------------------------------------------------------------------------------------- */
 

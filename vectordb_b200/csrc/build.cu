@@ -73,7 +73,9 @@ __global__ void select_edges_kernel(const int32_t* __restrict__ cand, const floa
   float* od = out_dist + v * out_stride;
   int nk = 0;
   if (keep_all_if_fits && n_valid <= out_degree) {
-    for (int i = lane; i < n_valid; i += 32) { const int s = order[i]; oi[i] = c[s]; od[i] = M[s]; }
+    // 1: in distance order; 2: in slot order (the valid candidates fill slots 1 .. n_valid, fill_cand_union_kernel), so
+    // the own list stays a prefix and the reverse candidates are appended to it
+    for (int i = lane; i < n_valid; i += 32) { const int s = keep_all_if_fits == 2 ? 1 + i : order[i]; oi[i] = c[s]; od[i] = M[s]; }
     nk = n_valid;
   } else {
     const int scan = min(n_valid, pool_cap);
@@ -135,22 +137,24 @@ __global__ void append_reverse_kernel(const int32_t* __restrict__ ids, const int
   rev_push(rev, rev_cap, rev_cnt, p, static_cast<int32_t>(v), salt);
 }
 
-// cand row for pass 2: [v, own list..., reverse candidates not already present...]
+// cand row for pass 2: [v, own list..., reverse candidates not already present...].  Row v of ids / cnt / rev is
+// vertex vids[v] (null: vertex v).
 __global__ void fill_cand_union_kernel(const int32_t* __restrict__ ids, const int32_t* __restrict__ cnt, int stride,
                                        const unsigned long long* __restrict__ rev, const int32_t* __restrict__ rev_cnt, int rev_cap,
-                                       int64_t v0, int batch, int32_t* __restrict__ cand) {
+                                       int64_t v0, int batch, int32_t* __restrict__ cand, const int32_t* __restrict__ vids) {
   const int64_t z = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (z >= batch) return;
   const int64_t v = v0 + z;
+  const int32_t id = vids ? vids[v] : static_cast<int32_t>(v);
   int32_t* c = cand + z * kC;
   int m = 0;
-  c[m++] = static_cast<int32_t>(v);
+  c[m++] = id;
   const int own = cnt[v];
   for (int j = 0; j < own && m < kC; ++j) c[m++] = ids[v * stride + j];
   const int nr = min(rev_cnt[v], rev_cap);
   for (int j = 0; j < nr && m < kC; ++j) {
     const int32_t u = rev_id(rev[v * rev_cap + j]);
-    bool dup = (u == v);
+    bool dup = (u == id);
     for (int t = 1; t <= own && !dup; ++t) dup = (c[t] == u);
     if (!dup) c[m++] = u;
   }
@@ -194,7 +198,7 @@ static int prune_pass(Index* ix, int64_t n, const unsigned long long* d_knn, int
                                                                                                 cand.as<int32_t>());
     } else {
       fill_cand_union_kernel<<<(batch + 127) / 128, 128, 0, ix->stream>>>(d_ids, d_cnt, stride, d_rev, d_rev_cnt, rev_cap,
-                                                                          v0, batch, cand.as<int32_t>());
+                                                                          v0, batch, cand.as<int32_t>(), nullptr);
     }
     EPS_TRY(launch_pair_tiles(ix, EPS_METRIC_L2, cand.as<int32_t>(), D.as<float>(), batch));
     if (getenv("EPS_DEBUG_SYNC")) EPS_CUDA(cudaStreamSynchronize(ix->stream));
@@ -210,17 +214,54 @@ static int prune_pass(Index* ix, int64_t n, const unsigned long long* d_knn, int
   return EPS_OK;
 }
 
-int install_csr(Index* ix, int64_t n, const int64_t* off, const int32_t* nb, int64_t e, int64_t nav) {
-  free_graph(ix);
-  EPS_TRY(ix->d_offsets.reserve((static_cast<size_t>(n) + 1) * 8));
-  EPS_TRY(ix->d_nbrs.reserve(std::max<size_t>(static_cast<size_t>(e), 1) * 4));
+int upload_csr(Index* ix, int64_t n, const int64_t* off, const int32_t* nb, int64_t e, int64_t nav) {
+  EPS_TRY(ix->d_offsets.grow((static_cast<size_t>(n) + 1) * 8, 0, ix->stream));
+  EPS_TRY(ix->d_nbrs.grow(std::max<size_t>(static_cast<size_t>(e), 1) * 4, 0, ix->stream));
   EPS_CUDA(cudaMemcpyAsync(ix->d_offsets, off, (static_cast<size_t>(n) + 1) * 8, cudaMemcpyHostToDevice, ix->stream));
   if (e > 0) EPS_CUDA(cudaMemcpyAsync(ix->d_nbrs, nb, static_cast<size_t>(e) * 4, cudaMemcpyHostToDevice, ix->stream));
   EPS_CUDA(cudaStreamSynchronize(ix->stream));
+  ix->d_ell.release();  // rebuilt by the next search
+  ix->init_L = 0;
+  ix->seed_rows_L = 0;
   ix->n_indexed = n;
   ix->n_edges = e;
   ix->nav = nav;
   return EPS_OK;
+}
+
+int install_csr(Index* ix, int64_t n, const int64_t* off, const int32_t* nb, int64_t e, int64_t nav) {
+  free_graph(ix);
+  return upload_csr(ix, n, off, nb, e, nav);
+}
+
+int graph_search_as(Index* ix, int metric, int width, const float* d_queries, int64_t nq, int64_t L,
+                    unsigned long long* d_queue, eps_stats* st) {
+  const int saved_metric = ix->metric, saved_width = ix->search_width, saved_screen = ix->graph_screen;
+  ix->metric = metric;
+  ix->search_width = width;
+  ix->graph_screen = EPS_GRAPH_SCREEN_OFF;
+  const int rc = graph_search(ix, d_queries, nq, L, d_queue, st);
+  ix->metric = saved_metric;
+  ix->search_width = saved_width;
+  ix->graph_screen = saved_screen;
+  return rc;
+}
+
+eps_build_params build_defaults(const eps_build_params* params) {
+  eps_build_params bp;
+  std::memset(&bp, 0, sizeof(bp));
+  if (params) bp = *params;
+  if (bp.knn_k <= 0) bp.knn_k = 100;          // Default_NSG_Config.knng
+  if (bp.out_degree <= 0) bp.out_degree = 50;  // .out_degree
+  if (bp.candidate_pool <= 0) bp.candidate_pool = 300;
+  if (bp.search_length <= 0) bp.search_length = 45;
+  if (bp.nnd_iters <= 0) bp.nnd_iters = 30;
+  if (bp.nnd_sample <= 0) bp.nnd_sample = 32;
+  if (bp.nnd_delta <= 0.f) bp.nnd_delta = 0.001f;
+  if (bp.exact_knn_below <= 0) bp.exact_knn_below = 60000;
+  if (bp.min_degree <= 0) bp.min_degree = 32;
+  if (bp.alpha <= 0.f) bp.alpha = 1.0f;
+  return bp;
 }
 
 ConnRepair::ConnRepair(int64_t n_, const int32_t* lists_, const int32_t* cnt_, int stride_)
@@ -233,7 +274,7 @@ void ConnRepair::flood(int32_t root) {
   while (!stack.empty()) {
     const int32_t u = stack.back();
     stack.pop_back();
-    const int32_t* row = &lists[static_cast<size_t>(u) * stride];
+    const int32_t* row = row_of(u);
     for (int j = 0; j < cnt[u]; ++j) {
       const int32_t w = row[j];
       if (!seen[w]) { seen[w] = 1; ++linked; stack.push_back(w); }
@@ -288,28 +329,64 @@ void ConnRepair::flatten(int64_t nav, std::vector<int64_t>* off, std::vector<int
   nb->assign(static_cast<size_t>(e), 0);
   for (int64_t v = 0; v < n; ++v) {
     int64_t o = (*off)[v];
-    for (int j = 0; j < cnt[v]; ++j) (*nb)[o++] = lists[static_cast<size_t>(v) * stride + j];
+    const int32_t* row = row_of(v);
+    for (int j = 0; j < cnt[v]; ++j) (*nb)[o++] = row[j];
     for (int32_t w : extra[v]) (*nb)[o++] = w;
   }
 }
 
+// Steps 3 and 4 of the connectivity repair, over the installed graph: in vertex order, every vertex rep has not
+// reached is searched for with its own row (L2, width 4, beam Ls, unscreened) and attached to the nearest linked vertex
+// of that search's pool, else to a random linked vertex; the attachments are floods of rep.
+int repair_by_search(Index* ix, ConnRepair* rep, int64_t Ls, uint64_t* rng, eps_stats* st) {
+  const int64_t n = rep->n;
+  std::vector<uint8_t>& seen = rep->seen;
+  std::vector<int32_t> unl;
+  for (int64_t v = 0; v < n; ++v) if (!seen[v]) unl.push_back(static_cast<int32_t>(v));
+  const int64_t chunk = 32768;
+  DevBuf d_ids, d_q, d_queue;
+  EPS_TRY(d_ids.reserve(static_cast<size_t>(chunk) * 4));
+  EPS_TRY(d_q.reserve(static_cast<size_t>(chunk) * ix->dim * 4));
+  EPS_TRY(d_queue.reserve(static_cast<size_t>(chunk) * Ls * 8));
+  std::vector<unsigned long long> h_pool(static_cast<size_t>(chunk) * Ls);
+  for (size_t c0 = 0; c0 < unl.size(); c0 += static_cast<size_t>(chunk)) {
+    const int64_t cn = static_cast<int64_t>(std::min<size_t>(static_cast<size_t>(chunk), unl.size() - c0));
+    // many of this chunk's vertices may have been linked by earlier attachments: search only the rest
+    std::vector<int32_t> todo;
+    for (int64_t i = 0; i < cn; ++i) if (!seen[unl[c0 + i]]) todo.push_back(unl[c0 + i]);
+    if (todo.empty()) continue;
+    const int64_t tn = static_cast<int64_t>(todo.size());
+    EPS_CUDA(cudaMemcpyAsync(d_ids.p, todo.data(), static_cast<size_t>(tn) * 4, cudaMemcpyHostToDevice, ix->stream));
+    EPS_TRY(gather_rows(ix, d_ids.as<int32_t>(), tn, d_q.as<float>()));
+    EPS_TRY(graph_search_as(ix, EPS_METRIC_L2, 4, d_q.as<float>(), tn, Ls, d_queue.as<unsigned long long>(), st));
+    ix->graph_counters_pending = false;
+    EPS_CUDA(cudaMemcpyAsync(h_pool.data(), d_queue.p, static_cast<size_t>(tn) * Ls * 8, cudaMemcpyDeviceToHost, ix->stream));
+    EPS_CUDA(cudaStreamSynchronize(ix->stream));
+    for (int64_t i = 0; i < tn; ++i) {
+      const int32_t u = todo[i];
+      if (seen[u]) continue;  // reached through an earlier attachment of this chunk
+      int32_t root = -1;
+      const unsigned long long* pool = &h_pool[static_cast<size_t>(i) * Ls];
+      for (int64_t j = 0; j < Ls; ++j) {  // 3. nearest linked vertex of the search pool (:757-766)
+        if ((pool[j] & kKeyMask) == kKeyInf) break;
+        const int32_t w = static_cast<int32_t>(key_id(pool[j]));
+        if (w != u && seen[w]) { root = w; break; }
+      }
+      if (root < 0) { rep->attach_random(u, rng); continue; }  // 4.
+      rep->extra[root].push_back(u);  // nsg[root].push_back(id) (:774), may exceed out_degree (Q11)
+      rep->flood(u);
+    }
+  }
+  return EPS_OK;
+}
+
 int build_graph(Index* ix, int64_t n, const eps_build_params* params) {
-  eps_build_params bp;
-  std::memset(&bp, 0, sizeof(bp));
-  if (params) bp = *params;
-  if (bp.knn_k <= 0) bp.knn_k = 100;          // Default_NSG_Config.knng
-  if (bp.out_degree <= 0) bp.out_degree = 50;  // .out_degree
-  if (bp.candidate_pool <= 0) bp.candidate_pool = 300;
-  if (bp.search_length <= 0) bp.search_length = 45;
-  if (bp.nnd_iters <= 0) bp.nnd_iters = 30;
-  if (bp.nnd_sample <= 0) bp.nnd_sample = 32;
-  if (bp.nnd_delta <= 0.f) bp.nnd_delta = 0.001f;
-  if (bp.exact_knn_below <= 0) bp.exact_knn_below = 60000;
+  const eps_build_params bp = build_defaults(params);
   if (n < 2 || n > ix->n_rows) return fail(EPS_ERR_INVALID_ARGUMENT, "build: n out of range");
   if (n >= (1ll << 31)) return fail(EPS_ERR_UNSUPPORTED, "build: more than 2^31 rows per shard");
   const int R = std::min<int>(bp.out_degree, 64);
-  const int min_deg = std::min<int>(bp.min_degree > 0 ? bp.min_degree : 32, R);
-  const float alpha = bp.alpha > 0.f ? bp.alpha : 1.0f;
+  const int min_deg = std::min<int>(bp.min_degree, R);
+  const float alpha = bp.alpha;
   const int K = static_cast<int>(std::min<int64_t>(std::min<int>(bp.knn_k, kC - 1), n - 1));
   eps_stats st;
   std::memset(&st, 0, sizeof(st));
@@ -416,10 +493,7 @@ int build_graph(Index* ix, int64_t n, const eps_build_params* params) {
   {
     rep.flood(static_cast<int32_t>(nav));
     rep.attach_from_knn(h_knn.data(), K);  // steps 1 and 2
-    std::vector<uint8_t>& seen = rep.seen;
     if (rep.linked < n) {
-      std::vector<int32_t> unl;
-      for (int64_t v = 0; v < n; ++v) if (!seen[v]) unl.push_back(static_cast<int32_t>(v));
       // install the un-repaired graph for the batched searches
       {
         std::vector<int64_t> off0(static_cast<size_t>(n) + 1);
@@ -431,50 +505,8 @@ int build_graph(Index* ix, int64_t n, const eps_build_params* params) {
         EPS_TRY(install_csr(ix, n, off0.data(), nb0.data(), e0, nav));
       }
       const int64_t Ls = std::min<int64_t>(n, std::max<int>(64, bp.search_length));
-      const int64_t chunk = 32768;
-      DevBuf d_ids, d_q, d_queue;
-      EPS_TRY(d_ids.reserve(static_cast<size_t>(chunk) * 4));
-      EPS_TRY(d_q.reserve(static_cast<size_t>(chunk) * ix->dim * 4));
-      EPS_TRY(d_queue.reserve(static_cast<size_t>(chunk) * Ls * 8));
-      std::vector<unsigned long long> h_pool(static_cast<size_t>(chunk) * Ls);
-      const int saved_metric = ix->metric, saved_width = ix->search_width;
       uint64_t rng = 0x9E3779B97F4A7C15ull ^ static_cast<uint64_t>(bp.seed);
-      int rc = EPS_OK;
-      for (size_t c0 = 0; c0 < unl.size() && rc == EPS_OK; c0 += static_cast<size_t>(chunk)) {
-        const int64_t cn = static_cast<int64_t>(std::min<size_t>(static_cast<size_t>(chunk), unl.size() - c0));
-        // many of this chunk's vertices may have been linked by earlier attachments: search only the rest
-        std::vector<int32_t> todo;
-        for (int64_t i = 0; i < cn; ++i) if (!seen[unl[c0 + i]]) todo.push_back(unl[c0 + i]);
-        if (todo.empty()) continue;
-        const int64_t tn = static_cast<int64_t>(todo.size());
-        ix->metric = EPS_METRIC_L2;
-        ix->search_width = 4;
-        rc = cudaMemcpyAsync(d_ids.p, todo.data(), static_cast<size_t>(tn) * 4, cudaMemcpyHostToDevice, ix->stream) == cudaSuccess ? EPS_OK : fail(EPS_ERR_CUDA, "repair: id upload failed");
-        if (rc == EPS_OK) rc = gather_rows(ix, d_ids.as<int32_t>(), tn, d_q.as<float>());
-        if (rc == EPS_OK) rc = graph_search(ix, d_q.as<float>(), tn, Ls, d_queue.as<unsigned long long>(), &st);
-        ix->metric = saved_metric;
-        ix->search_width = saved_width;
-        if (rc == EPS_OK && cudaMemcpyAsync(h_pool.data(), d_queue.p, static_cast<size_t>(tn) * Ls * 8, cudaMemcpyDeviceToHost, ix->stream) != cudaSuccess)
-          rc = fail(EPS_ERR_CUDA, "repair: pool download failed");
-        if (rc == EPS_OK && cudaStreamSynchronize(ix->stream) != cudaSuccess) rc = fail(EPS_ERR_CUDA, "repair: search failed");
-        if (rc != EPS_OK) break;
-        for (int64_t i = 0; i < tn; ++i) {
-          const int32_t u = todo[i];
-          if (seen[u]) continue;  // reached through an earlier attachment of this chunk
-          int32_t root = -1;
-          const unsigned long long* pool = &h_pool[static_cast<size_t>(i) * Ls];
-          for (int64_t j = 0; j < Ls; ++j) {  // 3. nearest linked vertex of the search pool (:757-766)
-            if ((pool[j] & kKeyMask) == kKeyInf) break;
-            const int32_t w = static_cast<int32_t>(key_id(pool[j]));
-            if (w != u && seen[w]) { root = w; break; }
-          }
-          if (root < 0) { rep.attach_random(u, &rng); continue; }  // 4.
-          rep.extra[root].push_back(u);  // nsg[root].push_back(id) (:774), may exceed out_degree (Q11)
-          rep.flood(u);
-        }
-      }
-      ix->graph_counters_pending = false;
-      if (rc != EPS_OK) return rc;
+      EPS_TRY(repair_by_search(ix, &rep, Ls, &rng, &st));
     }
   }
   std::vector<int64_t> off;

@@ -49,6 +49,14 @@ int Mem::grow(size_t bytes, size_t keep, cudaStream_t s) {
   return EPS_OK;
 }
 
+void Mem::swap(Mem& o) {
+  std::swap(p, o.p);
+  std::swap(cap, o.cap);
+  std::swap(owns, o.owns);
+  ++gen;
+  ++o.gen;
+}
+
 void Mem::release() {
   if (p && owns) {
     if (host) cudaFreeHost(p);
@@ -580,6 +588,20 @@ int eps_index_build(eps_index* h, int64_t n, const eps_build_params* params) {
   EPS_TRY(eps::build_graph(ix, n, params));
   eps::ensure_sketch(ix);
   return EPS_OK;
+}
+
+int eps_index_extend_graph(eps_index* h, int64_t n, const eps_build_params* params) {
+  Index* ix = reinterpret_cast<Index*>(h);
+  if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");
+  EPS_TRY(eps::dense_only(ix));
+  EPS_TRY(check_mutable(ix));
+  if (ix->n_indexed == 0) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "extend_graph: no graph installed (build one with eps_index_build)");
+  if (n < ix->n_indexed) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "extend_graph: n below the indexed rows");
+  if (n >= (1ll << 31)) return eps::fail(EPS_ERR_UNSUPPORTED, "extend_graph: more than 2^31 rows per shard");
+  if (n > ix->n_rows) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "extend_graph: n above the mirrored rows");
+  if (n == ix->n_indexed) return EPS_OK;
+  EPS_TRY(eps::check_device(ix->device));
+  return eps::extend_graph(ix, n, params);
 }
 
 int eps_index_get_graph(eps_index* h, int64_t* n_indexed, int64_t* n_edges, int64_t* offsets, int64_t* nbrs,

@@ -58,7 +58,6 @@
 
 namespace eps {
 
-constexpr int kEll = 64;        // adjacency ids per fixed-stride row
 constexpr int kMaxW = 8;        // candidates picked per iteration (upper bound)
 constexpr int kMaxS = 8;        // ring slots per consumer warp (upper bound)
 constexpr int kMaxR = 24;       // ring slots (upper bound: 3 consumer warps x kMaxS)

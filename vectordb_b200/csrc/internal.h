@@ -27,6 +27,8 @@ struct Mem {
   // Room for `bytes`, keeping the first `keep` (a device-to-device copy on s); the old memory is freed last, so a
   // failure leaves the buffer as it was.
   int grow(size_t bytes, size_t keep, cudaStream_t s);
+  // Exchange the memory of two buffers of the same kind (both device or both host).
+  void swap(Mem& o);
   void release();
   void alias(void* q, size_t bytes);
   template <typename T>
@@ -257,6 +259,7 @@ int prepare_init_ids(Index* ix, int64_t L);
 int graph_launch_prologue(Index* ix, int64_t L, const char* who, int* Lp);
 // Reserves and zeroes the counter block of a launch of nq queries (graph_search.cuh, GraphCounter).
 int graph_counters(Index* ix, int64_t nq);
+constexpr int kEll = 64;  // adjacency ids per fixed-stride (ELL) row
 int ensure_ell(Index* ix, uint64_t* launches);  // fixed-stride adjacency of the installed graph (built once)
 // out[i] = row d_ids[i] of the table (contiguous copy; used for seed rows and for the build's repair searches)
 int gather_rows(Index* ix, const int32_t* d_ids, int64_t n, float* d_out);
@@ -305,9 +308,18 @@ int merge_shards(int device, cudaStream_t stream, const int64_t* d_ids, const fl
                  int64_t dist_stride = 0);
 
 // ---- build.cu ------------------------------------------------------------------------------
+// The caller's build parameters with every unset (<= 0) field at its default.
+eps_build_params build_defaults(const eps_build_params* params);
 int build_graph(Index* ix, int64_t n, const eps_build_params* params);
 // Install a host CSR (int64 offsets, int32 ids) as the index's graph, dropping everything derived from the old one.
 int install_csr(Index* ix, int64_t n, const int64_t* off, const int32_t* nb, int64_t e, int64_t nav);
+// Replace the installed CSR with a host CSR and drop the adjacency table and seed set; the sketch (basis and row
+// sketches) is kept: the caller keeps the row sketches covering [0, n).
+int upload_csr(Index* ix, int64_t n, const int64_t* off, const int32_t* nb, int64_t e, int64_t nav);
+// graph_search with the metric and width given and the screen off, the handle's settings restored on every path
+// (the build's pools: they must not depend on, or count in, the screen of the searches the caller runs).
+int graph_search_as(Index* ix, int metric, int width, const float* d_queries, int64_t nq, int64_t L,
+                    unsigned long long* d_queue, eps_stats* st);
 
 // Connectivity repair of a build (CheckConnectivity, nsg.cpp:687-775) on host lists: the integer-only steps.
 // lists: [n x stride] out-neighbours, cnt[v] of them valid; knn: [n x K] sorted keys (kKeyInf padded).
@@ -316,6 +328,8 @@ struct ConnRepair {
   const int32_t* lists;
   const int32_t* cnt;
   int stride;
+  const int64_t* off = nullptr;  // set: lists is a CSR neighbour array and row u starts at off[u]
+  const int32_t* row_of(int64_t u) const { return lists + (off ? off[u] : u * stride); }
   std::vector<uint8_t> seen;
   std::vector<int32_t> stack;
   int64_t linked = 0;
@@ -330,6 +344,12 @@ struct ConnRepair {
   // entries become out-neighbours of nav; flatten lists + extra edges to the reference CSR
   void flatten(int64_t nav, std::vector<int64_t>* off, std::vector<int32_t>* nb);
 };
+// Steps 3 and 4 of the repair over the installed graph (rng: the LCG state of step 4).
+int repair_by_search(Index* ix, ConnRepair* rep, int64_t Ls, uint64_t* rng, eps_stats* st);
+
+// ---- extend.cu -----------------------------------------------------------------------------
+// Link rows [n_indexed, n) into the installed dense graph (eps_index_extend_graph); the caller has validated n.
+int extend_graph(Index* ix, int64_t n, const eps_build_params* params);
 
 // ---- like.cu -------------------------------------------------------------------------------
 // Append codes [first_code, first_code + count) to the dictionary mirror (eps_index_append_string_dictionary).

@@ -119,4 +119,14 @@ inline int launch_pair_tiles(Index* ix, int metric, const int32_t* d_cand, float
   return EPS_OK;
 }
 
+// Selection kernels of the build (build.cu), also run by the extension (extend.cu).
+__global__ void select_edges_kernel(const int32_t* __restrict__ cand, const float* __restrict__ D, int batch,
+                                    int out_degree, int pool_cap, int keep_all_if_fits, int min_degree, float alpha,
+                                    int64_t v_base,
+                                    int32_t* __restrict__ out_ids, float* __restrict__ out_dist,
+                                    int32_t* __restrict__ out_cnt, int out_stride);
+__global__ void fill_cand_union_kernel(const int32_t* __restrict__ ids, const int32_t* __restrict__ cnt, int stride,
+                                       const unsigned long long* __restrict__ rev, const int32_t* __restrict__ rev_cnt, int rev_cap,
+                                       int64_t v0, int batch, int32_t* __restrict__ cand, const int32_t* __restrict__ vids);
+
 }  // namespace eps

@@ -93,6 +93,15 @@ class Index:
             setattr(bp, k, v)
         check(self.L.eps_index_build(self.h, int(n), C.byref(bp)))
 
+    def extend_graph(self, n, **params):
+        """Link rows [n_indexed, n) into the installed graph without a full rebuild (eps_index_extend_graph); params are
+        eps_build_params fields as for build (knn_k, out_degree, candidate_pool, search_length, min_degree, alpha,
+        seed).  n == n_indexed does nothing."""
+        bp = BuildParams()
+        for k, v in params.items():
+            setattr(bp, k, v)
+        check(self.L.eps_index_extend_graph(self.h, int(n), C.byref(bp)))
+
     def get_graph(self):
         n, e, nav = C.c_int64(), C.c_int64(), C.c_int64()
         check(self.L.eps_index_get_graph(self.h, C.byref(n), C.byref(e), None, None, C.byref(nav)))

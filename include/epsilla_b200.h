@@ -293,6 +293,11 @@ EPS_API int eps_merge_shards_device(int device, const int64_t* d_ids, const floa
  * caller has no distances: has_distance = false).  Output per query q: out_groups[q] groups in order of first
  * appearance, keys out_keys[q*limit + g], values out_values[(q*limit + g)*n_aggs + a] (double, like the reference's
  * aggregators).  HOST buffers in and out.
+ * INT keys follow the reference's (int64_t) cast as x86-64 computes it: a key that is NaN or lies outside
+ * [-2^63, 2^63) (a division by zero, +-inf, an int64 product that overflows) becomes INT64_MIN, so with int4 columns
+ * a = [0, 5, -5, 7, 0, 1, 2, 3] and b = [0, 0, 0, 2, 1, 1, 1, 1], "a / b" groups COUNT(*) as {0: 1, 1: 1, 2: 1, 3: 2,
+ * INT64_MIN: 3} and "a % b" as {0: 4, 1: 1, INT64_MIN: 3}.  A NaN DOUBLE key makes the reference fail
+ * (FacetExecutor::Project throws); the device's grouping of such keys is unspecified.
  * --------------------------------------------------------------------------------------------- */
 typedef struct eps_facet {
   const eps_filter_node* key_nodes;

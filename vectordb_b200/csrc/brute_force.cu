@@ -527,10 +527,10 @@ static int scan_setup(Index* ix, const ScanRequest& r, int64_t k, ScanSetup* s, 
   EPS_TRY(ix->s_dist.reserve(static_cast<size_t>(r.nq) * s->chunk * 4));
   s->D = ix->s_dist.as<float>();
   s->smem = (2 * static_cast<size_t>(k) + kSelBuf) * 8;
-  if (s->smem > 48 * 1024) {
-    EPS_CUDA(cudaFuncSetAttribute(bf_select_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(s->smem)));
-    EPS_CUDA(cudaFuncSetAttribute(bf_select_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(s->smem)));
-  }
+  // The 48 KB launch default bounds the dynamic AND the kernel's static shared memory (about 1 KB): a list of k = 1984 to
+  // 2048 keys fits 48 KB alone but not with it.  Setting the limit on every call needs no guess at the static size.
+  EPS_CUDA(cudaFuncSetAttribute(bf_select_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(s->smem)));
+  EPS_CUDA(cudaFuncSetAttribute(bf_select_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(s->smem)));
   return EPS_OK;
 }
 

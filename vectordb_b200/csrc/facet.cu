@@ -6,7 +6,8 @@
 //
 // Device mapping, batched over nq result lists:
 //   facet_eval_kernel   one thread per (query, result): key and aggregate inputs through the same program evaluator
-//                       as the filters (filter.cuh); an INT key is truncated like the reference's (int64_t) cast, a
+//                       as the filters (filter.cuh); an INT key is truncated like the reference's (int64_t) cast
+//                       (int_key: NaN and out-of-range keys become INT64_MIN), a
 //                       BOOL key is LogicalEvaluate, a STRING key is the row's dictionary code;
 //   facet_group_kernel  one warp per query: a result is a group leader if no earlier result has its key; leaders
 //                       reduce their group sequentially in result order (the same order the reference adds values
@@ -33,6 +34,15 @@ struct FacetArgs {
   int64_t* out_groups;     // [nq]
 };
 
+// (int64_t)(NumEvaluate(..)) of an INT key (:272) as the reference computes it on x86-64 (cvttsd2si): NaN and every value
+// outside [-2^63, 2^63) become INT64_MIN.  The device's own conversion (cvt.rzi.s64.f64) saturates +inf and values of
+// 2^63 and above to INT64_MAX instead.
+__device__ __forceinline__ double int_key(double v) {
+  constexpr double kTwo63 = 9223372036854775808.0;
+  if (!(v >= -kTwo63 && v < kTwo63)) return -kTwo63;
+  return static_cast<double>(static_cast<long long>(v));
+}
+
 __global__ void facet_eval_kernel(FacetArgs a) {
   const int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
   if (t >= static_cast<int64_t>(a.nq) * a.limit) return;
@@ -48,7 +58,7 @@ __global__ void facet_eval_kernel(FacetArgs a) {
     key = bv ? 1.0 : 0.0;
   } else {
     key = value_eval(a.progs[0], a.attrs, a.attr_stride, row, dist);
-    if (a.key_type == VT_INT) key = static_cast<double>(static_cast<long long>(key));  // (int64_t)(NumEvaluate(..)) (:272)
+    if (a.key_type == VT_INT) key = int_key(key);
   }
   a.keys[t] = key;
   for (int g = 0; g < a.n_aggs; ++g) a.vals[t * a.n_aggs + g] = value_eval(a.progs[1 + g], a.attrs, a.attr_stride, row, dist);

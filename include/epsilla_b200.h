@@ -395,6 +395,27 @@ EPS_API int eps_search_sparse_batch(eps_index* ix, int64_t nq, const int64_t* q_
 #define EPS_SPARSE_SEARCH_GRAPH 1  /* the reference's branch rule: graph search + tail scan where it searches its graph */
 EPS_API int eps_index_set_sparse_search(eps_index* ix, int mode);
 
+/* Inverted index of a sparse IP or cosine index: per-term posting lists of the rows [0, n).
+ * What it does to results: nothing; it is not a search mode.  Every exact sparse scan a search call runs (the
+ * EPS_SPARSE_SEARCH_SCAN default; the brute-force, prefilter and force_brute branches of graph mode; the tail scan of
+ * graph mode) computes the distances of the covered rows from the postings and merges the uncovered rows [n, rows) as
+ * before, into the same distance tile.  Each covered row's matched products row[i] * query[i] are added in increasing
+ * index order from 0, in fp32 without FMA, as the merge adds them (db/vector.cpp:7-47), so the distances are bitwise
+ * those of the scan: ids, distances, counts and the n_dist / n_seed / n_expand / n_edges counters are what they are
+ * without the index.  Only kernel_launches and the timings change.
+ * Appends: rows appended after the build are scanned until the caller builds again, the way the graph's tail is.
+ * n = 0 drops the index.  A build replaces the previous index only once it has succeeded; a refused or failed call
+ * leaves the previous index as it was.  Refusals: an L2 index, EPS_ERR_UNSUPPORTED (its merged order also adds the
+ * row-only and query-only terms); a null or dense index, n < 0, n above the mirrored rows, a view, or an index with live
+ * views, EPS_ERR_INVALID_ARGUMENT.  Views created after the build share the index; a detached view has none.
+ * Device memory: 8 B per posting (one per element of the covered rows) plus 12 B per distinct index.  The build needs,
+ * while it runs, 16 B more per posting (sort keys and a second value buffer) plus the sort's scratch, beside the
+ * previous index, which is freed when the new one is installed.  A search call adds 16 B per query element. */
+EPS_API int eps_index_build_sparse_inverted(eps_index* ix, int64_t n);
+/* Rows covered (0 = none), distinct terms, postings.  Any pointer may be NULL.  A null or dense index:
+ * EPS_ERR_INVALID_ARGUMENT. */
+EPS_API int eps_index_sparse_inverted_info(eps_index* ix, int64_t* n_rows, int64_t* n_terms, int64_t* n_postings);
+
 /* Raw stream handle (cudaStream_t) the index launches on, for callers that time with CUDA events. */
 EPS_API void* eps_index_stream(eps_index* ix);
 

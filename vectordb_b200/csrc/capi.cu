@@ -246,7 +246,8 @@ struct DenseBatch : QueryBatch {
 
 struct SparseBatch : QueryBatch {
   const SparseDist& dist;  // the caller's: a copy of the batch still points at it
-  explicit SparseBatch(const SparseDist& d) : dist(d) { scan.dist = &d; scan.nq = d.nq; }
+  // tile: the exact scan's producer, d itself or the inverted index's (the graph search always takes the raw queries)
+  SparseBatch(const SparseDist& d, const DistProducer& tile) : dist(d) { scan.dist = &tile; scan.nq = d.nq; }
   int graph(Index* ix, int64_t L, unsigned long long* d_queue, eps_stats* st) const override {
     return sparse_graph_search(ix, dist.q, dist.nq, L, d_queue, st);
   }
@@ -818,8 +819,33 @@ int eps_search_sparse_batch(eps_index* h, int64_t nq, const int64_t* q_offsets, 
   const eps::SparseDist dist(eps::SparseQueries{reinterpret_cast<const int64_t*>(d_q),
                                                 reinterpret_cast<const uint2*>(d_q + el_off),
                                                 reinterpret_cast<const float*>(d_q + nrm_off)}, nq);
-  return eps::search_to_host(ix, eps::SparseBatch(dist), nq, limit, filter, n_filter, out_ids, out_dists,
+  const eps::InvertedDist inv(dist, static_cast<int64_t>(qe.size()));
+  const eps::DistProducer& tile = ix->inv_rows > 0 ? static_cast<const eps::DistProducer&>(inv) : dist;
+  return eps::search_to_host(ix, eps::SparseBatch(dist, tile), nq, limit, filter, n_filter, out_ids, out_dists,
                              out_counts, stats);
+}
+
+int eps_index_build_sparse_inverted(eps_index* h, int64_t n) {
+  Index* ix = reinterpret_cast<Index*>(h);
+  if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");
+  if (!ix->sparse) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "inverted index on a dense index");
+  if (ix->metric == EPS_METRIC_L2)
+    return eps::fail(EPS_ERR_UNSUPPORTED, "inverted index on an L2 index: the L2 sum also adds the row-only and "
+                                          "query-only terms in merged index order, which posting lists cannot reproduce");
+  EPS_TRY(check_mutable(ix));
+  if (n < 0 || n > ix->n_rows) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "inverted index: n outside [0, mirrored rows]");
+  EPS_TRY(eps::check_device(ix->device));
+  return eps::build_sparse_inverted(ix, n);
+}
+
+int eps_index_sparse_inverted_info(eps_index* h, int64_t* n_rows, int64_t* n_terms, int64_t* n_postings) {
+  Index* ix = reinterpret_cast<Index*>(h);
+  if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");
+  if (!ix->sparse) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "inverted index info on a dense index");
+  if (n_rows) *n_rows = ix->inv_rows;
+  if (n_terms) *n_terms = ix->inv_terms;
+  if (n_postings) *n_postings = ix->inv_postings;
+  return EPS_OK;
 }
 
 int eps_merge_shards_device(int device, const int64_t* d_ids, const float* d_dists, int64_t n_shards, int64_t nq,

@@ -102,6 +102,25 @@ __device__ __forceinline__ float finish_metric(int metric, float acc) {
   return acc;
 }
 
+// Distance of a sparse (row, query) pair from its sequential fp32 accumulation (db/vector.cpp:7-100): the L2 sum as it
+// is, -dot, or 1 - dot / sqrt(rn * qn) with rn, qn the two squared norms.  A NaN becomes the one NaN with the sign bit
+// clear, which sorts after +inf.  The sparse scan and the inverted index both finish here, so their tiles cannot drift.
+template <int METRIC>
+__device__ __forceinline__ float sparse_finish(float acc, float rn, float qn) {
+  float d;
+  if (METRIC == EPS_METRIC_L2) {
+    d = acc;
+  } else if (METRIC == EPS_METRIC_IP) {
+    d = -acc;
+  } else {
+    // IEEE division and square root are called subroutines on sm_90; the call saves one register pair (the 8-byte
+    // stack frame -Xptxas -v reports for the scan's cosine instance), once per (row, query), outside the merge loop
+    d = __fsub_rn(1.0f, __fdiv_rn(acc, __fsqrt_rn(__fmul_rn(rn, qn))));
+  }
+  if (d != d) d = __uint_as_float(0x7fffffffu);
+  return d;
+}
+
 // Per-lane partial of one row against the query held in shared memory.
 // VEC4 path: dim % 4 == 0 and 16-byte aligned rows; lane l covers float4 chunks l, l+32, ...
 template <bool L2>

@@ -87,6 +87,13 @@ struct Table {
   DevArray<uint2> d_sp_elems;   // {index, value bits}, indices strictly increasing within a row
   DevArray<float> d_sp_norm2;   // [rows] sequential fp32 sum of squares of each row (cosine); its room is the row room
   int64_t sp_nnz = 0;
+  // inverted index of the sparse rows [0, inv_rows) (sparse_inverted.cu): the exact scan reads their distances from it
+  DevArray<uint32_t> d_inv_terms;  // [inv_terms] the distinct indices, ascending
+  DevArray<int64_t> d_inv_ptr;     // [inv_terms + 1] posting offsets of the terms
+  DevArray<uint2> d_inv_post;      // [inv_postings] {int32 row, float value bits}, rows ascending within a term
+  int64_t inv_rows = 0;            // rows covered (0: no index)
+  int64_t inv_terms = 0;
+  int64_t inv_postings = 0;
 
   // graph (ANNGraphSegment mirror)
   int64_t n_indexed = 0;
@@ -161,7 +168,7 @@ struct Index : Table, Config {
   // scratch
   DevBuf s_queries, s_dist, s_topk, s_topk2, s_pass, s_filter, s_vset, s_visited, s_vlog, s_queue, s_tail, s_out_ids, s_out_dists,
       s_out_counts, s_stats, s_misc, s_seed_rows, s_seed_dist, s_xnorm, s_qnorm, s_coarse, s_thr, s_cand, s_cand_cnt, s_bf16, s_qbf16, s_flags,
-      s_sparse_q, s_xnorm_max, s_like, s_like_jobs;
+      s_sparse_q, s_xnorm_max, s_like, s_like_jobs, s_inv_plan;
   int64_t bf16_rows = 0;         // rows converted into s_bf16 while it had generation bf16_gen
   uint64_t bf16_gen = 0;
   int64_t xnorm_rows = 0;        // rows whose |x|^2 is current in s_xnorm; s_xnorm_max holds the largest (float bits)
@@ -242,6 +249,20 @@ int pack_sparse(int64_t n, const int64_t* offsets, const int64_t* indices, const
 int sparse_append(Index* ix, int64_t first_row, int64_t n_rows, const int64_t* offsets, const int64_t* indices,
                   const float* values);
 int build_graph_sparse(Index* ix, int64_t n, const eps_build_params* params);
+
+// ---- sparse_inverted.cu --------------------------------------------------------------------
+// Posting lists of rows [0, n) of a sparse IP / cosine index (n = 0 drops them); the caller has validated ix and n.
+int build_sparse_inverted(Index* ix, int64_t n);
+// The sparse scan's distance tile with the rows [0, inv_rows) read from the posting lists, bitwise the tile of
+// SparseDist: each row's products are added in the query's index order, from 0, as sparse_dist_kernel adds them.
+// Rows at or above inv_rows go to SparseDist.  The queries' offsets start at 0 (q.ptr[0] = 0); n_elems = q.ptr[nq].
+struct InvertedDist : DistProducer {
+  SparseDist scan;
+  int64_t n_elems;
+  mutable bool planned = false;  // the query elements' posting ranges are in ix->s_inv_plan (one plan per call)
+  InvertedDist(const SparseDist& s, int64_t n_elems_) : scan(s), n_elems(n_elems_) {}
+  int launch(Index* ix, int metric, int64_t row_start, int64_t n, float* D, int64_t ldd, uint64_t* launches) const override;
+};
 
 // ---- sparse_graph.cu -----------------------------------------------------------------------
 // graph_search for sparse queries at width 1 (the reference's sequential order): d_queue [nq x L] sorted keys.

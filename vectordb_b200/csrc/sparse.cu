@@ -112,19 +112,9 @@ __global__ void __launch_bounds__(kSpWarps * 32) sparse_dist_kernel(
           acc = __fadd_rn(acc, __fmul_rn(y, y));
         }
       }
-      float d;
-      if (METRIC == EPS_METRIC_L2) {
-        d = acc;
-      } else if (METRIC == EPS_METRIC_IP) {
-        d = -acc;
-      } else {
-        const float rn = __shfl_sync(kFull, my_rn, j);
-        // IEEE division and square root are called subroutines on sm_90; the call saves one register pair (the
-        // 8-byte stack frame -Xptxas -v reports for this instance only), once per (row, query), outside the merge loop
-        d = __fsub_rn(1.0f, __fdiv_rn(acc, __fsqrt_rn(__fmul_rn(rn, qn))));
-      }
-      if (d != d) d = __uint_as_float(0x7fffffffu);  // one NaN, with the sign bit clear: it sorts after +inf
-      my[j * 33 + lane] = d;
+      float rn = 0.f;
+      if (METRIC == EPS_METRIC_COSINE) rn = __shfl_sync(kFull, my_rn, j);
+      my[j * 33 + lane] = sparse_finish<METRIC>(acc, rn, qn);
     }
     __syncwarp();
     if (lane < rows_here)

@@ -237,7 +237,8 @@ SPARSE_SEARCH_MODES = {"scan": 0, "graph": 1}
 class SparseIndex(Index):
     """Device mirror of one sparse-vector field (eps_index_create_sparse): rows are appended as CSR.  Searches are exact
     scans by default; set_search_mode("graph") searches the graph that build() installed where the reference would
-    (n_indexed >= 512, no prefilter / force_brute), with the reference's results at IntraQueryThreads = 1.  Config,
+    (n_indexed >= 512, no prefilter / force_brute), with the reference's results at IntraQueryThreads = 1.
+    build_inverted() gives an IP or cosine index posting lists that the exact scans read, with the same results.  Config,
     deleted bits, attributes, string codes and dictionary, facets, build and get_graph work as on Index."""
 
     def __init__(self, metric, dim, capacity=0, device=0):
@@ -268,6 +269,18 @@ class SparseIndex(Index):
     def set_search_mode(self, mode):
         """"scan" (default): exact scan always; "graph": the reference's branch rule (eps_index_set_sparse_search)."""
         check(self.L.eps_index_set_sparse_search(self.h, SPARSE_SEARCH_MODES.get(mode, mode)))
+
+    def build_inverted(self, n=None):
+        """Posting lists of rows [0, n) (None: every mirrored row; 0 drops them) for an IP or cosine index
+        (eps_index_build_sparse_inverted).  Results do not change; the exact scans read the covered rows' distances
+        from the postings.  Rows appended later are scanned until the next build."""
+        check(self.L.eps_index_build_sparse_inverted(self.h, self.rows if n is None else int(n)))
+
+    def inverted_info(self):
+        """dict(rows=rows covered (0: no index), terms=distinct indices, postings=posting entries)."""
+        r, t, p = C.c_int64(0), C.c_int64(0), C.c_int64(0)
+        check(self.L.eps_index_sparse_inverted_info(self.h, C.byref(r), C.byref(t), C.byref(p)))
+        return dict(rows=int(r.value), terms=int(t.value), postings=int(p.value))
 
     def append(self, rows, first_row=None):
         """Append CSR rows (scipy CSR or (offsets, indices, values)) after the rows already mirrored."""

@@ -265,6 +265,7 @@ def test_sparse_view_searches_concurrently(vdb):
     ix.config(500, 500, force_brute=True)
     want = ix.search(qs, 10)
     v = ix.view()
+    assert isinstance(v, vdb.SparseIndex)   # searches take CSR queries through eps_search_sparse_batch
     out = {}
     def run(name, index):
         out[name] = [index.search(qs, 10) for _ in range(4)]

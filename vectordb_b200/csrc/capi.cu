@@ -808,17 +808,9 @@ int eps_search_sparse_batch(eps_index* h, int64_t nq, const int64_t* q_offsets, 
   std::vector<float> qn;
   EPS_TRY(eps::pack_sparse(nq, q_offsets, q_indices, q_values, 0xffffffffll, 0, &qp, &qe, &qn));
   if (stats) EPS_CUDA(cudaEventRecord(ix->ev[0], ix->stream));
-  // one device block [ptr | norm2 | elems]
-  const size_t ptr_bytes = static_cast<size_t>(nq + 1) * 8, nrm_off = ptr_bytes,
-               el_off = nrm_off + ((static_cast<size_t>(nq) * 4 + 7) & ~static_cast<size_t>(7));
-  EPS_TRY(ix->s_sparse_q.reserve(el_off + qe.size() * 8));
-  unsigned char* d_q = ix->s_sparse_q.as<unsigned char>();
-  EPS_CUDA(cudaMemcpyAsync(d_q, qp.data(), ptr_bytes, cudaMemcpyHostToDevice, ix->stream));
-  EPS_CUDA(cudaMemcpyAsync(d_q + nrm_off, qn.data(), static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, ix->stream));
-  if (!qe.empty()) EPS_CUDA(cudaMemcpyAsync(d_q + el_off, qe.data(), qe.size() * 8, cudaMemcpyHostToDevice, ix->stream));
-  const eps::SparseDist dist(eps::SparseQueries{reinterpret_cast<const int64_t*>(d_q),
-                                                reinterpret_cast<const uint2*>(d_q + el_off),
-                                                reinterpret_cast<const float*>(d_q + nrm_off)}, nq);
+  eps::SparseQueries q;
+  EPS_TRY(eps::upload_sparse_queries(ix, qp, qe, qn, &ix->s_sparse_q, &q));
+  const eps::SparseDist dist(q, nq);
   const eps::InvertedDist inv(dist, static_cast<int64_t>(qe.size()));
   const eps::DistProducer& tile = ix->inv_rows > 0 ? static_cast<const eps::DistProducer&>(inv) : dist;
   return eps::search_to_host(ix, eps::SparseBatch(dist, tile), nq, limit, filter, n_filter, out_ids, out_dists,

@@ -102,9 +102,60 @@ __device__ __forceinline__ float finish_metric(int metric, float acc) {
   return acc;
 }
 
+// Sequential fp32 accumulation of one sparse row (v1) against the query elements q[qb, qe) (v2), in the reference's
+// order (db/vector.cpp:7-100): GetInnerProductDist and GetCosineDist add v1*v2 over the matching indices in increasing
+// index order; GetL2DistSqr adds over the MERGED index sequence (v1-v2)^2, v1^2 (row only) or v2^2 (query only).
+// vector.cpp is compiled -O3 with SSE2 only, so every sum is sequential fp32 without FMA: __fmul_rn / __fadd_rn keep
+// nvcc from contracting.  Feed the row's elements to add() in increasing index order, then take sum().  The sparse scan
+// and the sparse graph search both merge here, so their distances cannot drift.
+constexpr uint32_t kSparseEnd = 0xffffffffu;  // end-of-query sentinel: above every legal index (< dim < 2^32 - 1)
+
+template <int METRIC>
+struct SparseMerge {
+  const uint2* q;
+  int64_t qi, qe;
+  uint2 cur;  // q[qi], or the sentinel past the end
+  float acc = 0.f;
+  __device__ __forceinline__ SparseMerge(const uint2* q_, int64_t qb, int64_t qe_) : q(q_), qi(qb), qe(qe_) { load(); }
+  __device__ __forceinline__ void load() { cur = qi < qe ? q[qi] : make_uint2(kSparseEnd, 0u); }
+  __device__ __forceinline__ void add(uint32_t idx, float val) {
+    while (cur.x < idx) {  // query-only elements below the row's index
+      if (METRIC == EPS_METRIC_L2) {
+        const float y = __uint_as_float(cur.y);
+        acc = __fadd_rn(acc, __fmul_rn(y, y));
+      }
+      ++qi;
+      load();
+    }
+    if (cur.x == idx) {
+      const float y = __uint_as_float(cur.y);
+      if (METRIC == EPS_METRIC_L2) {
+        const float d = __fsub_rn(val, y);
+        acc = __fadd_rn(acc, __fmul_rn(d, d));
+      } else {
+        acc = __fadd_rn(acc, __fmul_rn(val, y));
+      }
+      ++qi;
+      load();
+    } else if (METRIC == EPS_METRIC_L2) {  // row-only element
+      acc = __fadd_rn(acc, __fmul_rn(val, val));
+    }
+  }
+  __device__ __forceinline__ float sum() {
+    if (METRIC == EPS_METRIC_L2) {
+      for (; qi < qe; ++qi) {  // query-only elements past the row's last index
+        const float y = __uint_as_float(q[qi].y);
+        acc = __fadd_rn(acc, __fmul_rn(y, y));
+      }
+    }
+    return acc;
+  }
+};
+
 // Distance of a sparse (row, query) pair from its sequential fp32 accumulation (db/vector.cpp:7-100): the L2 sum as it
 // is, -dot, or 1 - dot / sqrt(rn * qn) with rn, qn the two squared norms.  A NaN becomes the one NaN with the sign bit
-// clear, which sorts after +inf.  The sparse scan and the inverted index both finish here, so their tiles cannot drift.
+// clear, which sorts after +inf.  The sparse scan, the sparse graph search and the inverted index all finish here, so
+// their distances cannot drift.
 template <int METRIC>
 __device__ __forceinline__ float sparse_finish(float acc, float rn, float qn) {
   float d;

@@ -246,6 +246,10 @@ struct SparseDist : DistProducer {
 // ptr_base), elems and norm2.  Indices must be >= 0, < max_index and strictly increasing within a row.
 int pack_sparse(int64_t n, const int64_t* offsets, const int64_t* indices, const float* values, int64_t max_index,
                 int64_t ptr_base, std::vector<int64_t>* ptr, std::vector<uint2>* elems, std::vector<float>* norm2);
+// Reserve buf for a query set packed by pack_sparse (ptr_base 0) and enqueue its upload on ix->stream as one block
+// [ptr | norm2 | elems]; *q points into buf.
+int upload_sparse_queries(Index* ix, const std::vector<int64_t>& ptr, const std::vector<uint2>& elems,
+                          const std::vector<float>& norm2, DevBuf* buf, SparseQueries* q);
 int sparse_append(Index* ix, int64_t first_row, int64_t n_rows, const int64_t* offsets, const int64_t* indices,
                   const float* values);
 int build_graph_sparse(Index* ix, int64_t n, const eps_build_params* params);

@@ -5,9 +5,9 @@
 // Why the tile is bitwise the scan's: for IP and cosine the reference adds the matched products row[i] * query[i] in
 // increasing index order, from 0 (engine/db/vector.cpp:7-47).  inverted_score_kernel walks a query's elements in their
 // (increasing) index order and adds each term's posting value times the query value into a per-row fp32 accumulator
-// that starts at 0, with __fmul_rn / __fadd_rn: every row sees the same operations in the same order as in
-// sparse_dist_kernel, and both finish through sparse_finish.  A row that matches nothing keeps 0, as in the merge.
-// L2 cannot be served: its merged order also adds the row-only and query-only terms.
+// that starts at 0, with __fmul_rn / __fadd_rn: every row sees the same operations in the same order as in SparseMerge
+// (common.cuh), and the tile finishes through sparse_finish like every other sparse distance.  A row that matches
+// nothing keeps 0, as in the merge.  L2 cannot be served: its merged order also adds the row-only and query-only terms.
 //
 // Build: expand the CSR elements of rows [0, n) to (index, {row, value}) pairs, sort them by index with a stable radix
 // sort (rows stay ascending within a term), flag the first posting of each term and take the int64 exclusive sum of the

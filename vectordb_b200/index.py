@@ -25,6 +25,14 @@ def filter_nodes_array(nodes):
     return arr, n
 
 
+def _build_params(params):
+    """eps_build_params with the given fields set and the others 0."""
+    bp = BuildParams()
+    for k, v in params.items():
+        setattr(bp, k, v)
+    return bp
+
+
 class Stats(dict):
     @classmethod
     def from_struct(cls, s):
@@ -37,30 +45,32 @@ class Index:
     """Device mirror of one vector field of a TableSegmentMVP + its ANNGraphSegment + executor params."""
 
     def __init__(self, metric, dim, host_vectors=None, capacity=None, device=0):
+        if host_vectors is not None:
+            host_vectors = np.ascontiguousarray(host_vectors, np.float32)
+            assert host_vectors.ndim == 2 and host_vectors.shape[1] == dim
+            capacity = host_vectors.shape[0] if capacity is None else capacity
+        self._open(metric, dim, host_vectors, capacity, device,
+                   lambda h: self.L.eps_index_create(h, self.metric, self.dim, _p(self._host), self.capacity, device))
+
+    def _open(self, metric, dim, host, capacity, device, create):
+        """Field set-up of every constructor and view; create(handle pointer) makes the C handle."""
         self.L = load_library()
         self.metric = METRICS[metric] if isinstance(metric, str) else int(metric)
         self.dim = int(dim)
         self.device = device
-        self._host = None
-        if host_vectors is not None:
-            host_vectors = np.ascontiguousarray(host_vectors, np.float32)
-            assert host_vectors.ndim == 2 and host_vectors.shape[1] == dim
-            self._host = host_vectors
-            capacity = host_vectors.shape[0] if capacity is None else capacity
+        self._host = host
         self.capacity = int(capacity or 0)
-        h = C.c_void_p()
-        check(self.L.eps_index_create(C.byref(h), self.metric, self.dim, _p(self._host), self.capacity, device))
-        self.h = h
         self._keep = []
+        h = C.c_void_p()
+        check(create(C.byref(h)))
+        self.h = h
 
     def view(self):
         """Read-only view sharing this index's device data, with its own stream and scratch (eps_index_create_view):
         searches on the view overlap searches on the base.  Close the views before the base."""
-        v = Index.__new__(Index)
-        v.L, v.metric, v.dim, v.device, v._host, v.capacity, v._keep = self.L, self.metric, self.dim, self.device, None, self.capacity, []
-        h = C.c_void_p()
-        check(self.L.eps_index_create_view(self.h, C.byref(h)))
-        v.h = h
+        v = type(self).__new__(type(self))
+        v._open(self.metric, self.dim, None, self.capacity, self.device,
+                lambda h: self.L.eps_index_create_view(self.h, h))
         v._base = self  # keeps the base alive
         return v
 
@@ -88,19 +98,13 @@ class Index:
         check(self.L.eps_index_set_graph(self.h, int(n_indexed), _p(offsets), _p(nbrs), int(nav)))
 
     def build(self, n, **params):
-        bp = BuildParams()
-        for k, v in params.items():
-            setattr(bp, k, v)
-        check(self.L.eps_index_build(self.h, int(n), C.byref(bp)))
+        check(self.L.eps_index_build(self.h, int(n), C.byref(_build_params(params))))
 
     def extend_graph(self, n, **params):
         """Link rows [n_indexed, n) into the installed graph without a full rebuild (eps_index_extend_graph); params are
         eps_build_params fields as for build (knn_k, out_degree, candidate_pool, search_length, min_degree, alpha,
         seed).  n == n_indexed does nothing."""
-        bp = BuildParams()
-        for k, v in params.items():
-            setattr(bp, k, v)
-        check(self.L.eps_index_extend_graph(self.h, int(n), C.byref(bp)))
+        check(self.L.eps_index_extend_graph(self.h, int(n), C.byref(_build_params(params))))
 
     def get_graph(self):
         n, e, nav = C.c_int64(), C.c_int64(), C.c_int64()
@@ -171,13 +175,16 @@ class Index:
         if q.ndim == 1:
             q = q[None, :]
         nq = q.shape[0]
+        return self._search_host(self.L.eps_search_batch, (self.h, _p(q), nq), nq, limit, filter_nodes, want_stats)
+
+    def _search_host(self, fn, head, nq, limit, filter_nodes, want_stats):
+        """fn(*head, limit, filter, n_filter, ids, dists, counts, stats) into new host arrays: ids, dists, counts, Stats."""
         ids = np.empty((nq, limit), np.int64)
         dists = np.empty((nq, limit), np.float64)
         counts = np.empty(nq, np.int64)
         st = StatsStruct()
         arr, n = filter_nodes_array(filter_nodes)
-        check(self.L.eps_search_batch(self.h, _p(q), nq, int(limit), arr, n, _p(ids), _p(dists), _p(counts),
-                                      C.byref(st) if want_stats else None))
+        check(fn(*head, int(limit), arr, n, _p(ids), _p(dists), _p(counts), C.byref(st) if want_stats else None))
         return ids, dists, counts, Stats.from_struct(st)
 
     def search_device(self, d_queries_ptr, nq, limit, d_ids_ptr, d_dists_ptr, d_counts_ptr, filter_nodes=None,
@@ -242,25 +249,8 @@ class SparseIndex(Index):
     deleted bits, attributes, string codes and dictionary, facets, build and get_graph work as on Index."""
 
     def __init__(self, metric, dim, capacity=0, device=0):
-        self.L = load_library()
-        self.metric = METRICS[metric] if isinstance(metric, str) else int(metric)
-        self.dim = int(dim)
-        self.device = device
-        self._host = None
-        self.capacity = int(capacity or 0)
-        self._keep = []
-        h = C.c_void_p()
-        check(self.L.eps_index_create_sparse(C.byref(h), self.metric, self.dim, self.capacity, device))
-        self.h = h
-
-    def view(self):
-        v = SparseIndex.__new__(SparseIndex)
-        v.L, v.metric, v.dim, v.device, v._host, v.capacity, v._keep = self.L, self.metric, self.dim, self.device, None, self.capacity, []
-        h = C.c_void_p()
-        check(self.L.eps_index_create_view(self.h, C.byref(h)))
-        v.h = h
-        v._base = self
-        return v
+        self._open(metric, dim, None, capacity, device,
+                   lambda h: self.L.eps_index_create_sparse(h, self.metric, self.dim, self.capacity, device))
 
     @property
     def rows(self):
@@ -292,14 +282,8 @@ class SparseIndex(Index):
         """Search of CSR queries (eps_search_sparse_batch), by the mode of set_search_mode.  Returns ids [nq,limit], dists float64, counts, Stats."""
         off, idx, val = as_csr(queries)
         nq = off.size - 1
-        ids = np.empty((nq, limit), np.int64)
-        dists = np.empty((nq, limit), np.float64)
-        counts = np.empty(nq, np.int64)
-        st = StatsStruct()
-        arr, n = filter_nodes_array(filter_nodes)
-        check(self.L.eps_search_sparse_batch(self.h, nq, _p(off), _p(idx), _p(val), int(limit), arr, n, _p(ids), _p(dists),
-                                             _p(counts), C.byref(st) if want_stats else None))
-        return ids, dists, counts, Stats.from_struct(st)
+        return self._search_host(self.L.eps_search_sparse_batch, (self.h, nq, _p(off), _p(idx), _p(val)), nq, limit,
+                                 filter_nodes, want_stats)
 
 
 def normalize(vectors, device=0):

@@ -384,7 +384,9 @@ EPS_API int eps_index_append_sparse_rows(eps_index* ix, int64_t first_row, int64
  * unspecified): NaN distances sort after every number.
  * eps_index_build on a sparse index installs the exact out_degree-NN lists (field metric, self excluded), the L2
  * nearest row to the reference's sparse centre (nsg.cpp:120-135) as navigation point, and repair edges that make every
- * row reachable from it.  HOST buffers in and out. */
+ * row reachable from it.  A build on an index with posting lists (eps_index_build_sparse_inverted) reads the covered
+ * rows' kNN distances from them, bitwise the merge's, so the graph is the same; the build neither creates nor drops
+ * posting lists.  HOST buffers in and out. */
 EPS_API int eps_search_sparse_batch(eps_index* ix, int64_t nq, const int64_t* q_offsets, const int64_t* q_indices,
                                     const float* q_values, int64_t limit, const eps_filter_node* filter, int64_t n_filter,
                                     int64_t* out_ids, double* out_dists, int64_t* out_counts, eps_stats* stats);
@@ -410,7 +412,8 @@ EPS_API int eps_index_set_sparse_search(eps_index* ix, int mode);
  * views, EPS_ERR_INVALID_ARGUMENT.  Views created after the build share the index; a detached view has none.
  * Device memory: 8 B per posting (one per element of the covered rows) plus 12 B per distinct index.  The build needs,
  * while it runs, 16 B more per posting (sort keys and a second value buffer) plus the sort's scratch, beside the
- * previous index, which is freed when the new one is installed.  A search call adds 16 B per query element. */
+ * previous index, which is freed when the new one is installed.  A search call adds 16 B per query element; a graph
+ * build (eps_index_build) 16 B per element of its largest 8192-row query chunk. */
 EPS_API int eps_index_build_sparse_inverted(eps_index* ix, int64_t n);
 /* Rows covered (0 = none), distinct terms, postings.  Any pointer may be NULL.  A null or dense index:
  * EPS_ERR_INVALID_ARGUMENT. */

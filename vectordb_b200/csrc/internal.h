@@ -259,12 +259,15 @@ int build_graph_sparse(Index* ix, int64_t n, const eps_build_params* params);
 int build_sparse_inverted(Index* ix, int64_t n);
 // The sparse scan's distance tile with the rows [0, inv_rows) read from the posting lists, bitwise the tile of
 // SparseDist: each row's products are added in the query's index order, from 0, as sparse_dist_kernel adds them.
-// Rows at or above inv_rows go to SparseDist.  The queries' offsets start at 0 (q.ptr[0] = 0); n_elems = q.ptr[nq].
+// Rows at or above inv_rows go to SparseDist.  The queries' elements are [elem_base, elem_base + n_elems) of q.elems
+// (elem_base = q.ptr[0], n_elems = q.ptr[nq] - elem_base): 0 for an uploaded query set, the chunk's first element when
+// the build's queries are rows of the mirror itself.  The plan holds those elements only.
 struct InvertedDist : DistProducer {
   SparseDist scan;
-  int64_t n_elems;
+  int64_t n_elems, elem_base;
   mutable bool planned = false;  // the query elements' posting ranges are in ix->s_inv_plan (one plan per call)
-  InvertedDist(const SparseDist& s, int64_t n_elems_) : scan(s), n_elems(n_elems_) {}
+  InvertedDist(const SparseDist& s, int64_t n_elems_, int64_t elem_base_ = 0)
+      : scan(s), n_elems(n_elems_), elem_base(elem_base_) {}
   int launch(Index* ix, int metric, int64_t row_start, int64_t n, float* D, int64_t ldd, uint64_t* launches) const override;
 };
 

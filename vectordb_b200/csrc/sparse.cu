@@ -206,17 +206,24 @@ int build_graph_sparse(Index* ix, int64_t n, const eps_build_params* params) {
   const int seed = params ? params->seed : 0;
   eps_stats st;
   std::memset(&st, 0, sizeof(st));
-  // ---- kNN lists: the rows as queries of the exact scan ----
+  std::vector<int64_t> ptr(static_cast<size_t>(n) + 1);  // the rows' element offsets (ptr[0] = 0)
+  if (cudaMemcpy(ptr.data(), ix->d_sp_ptr, ptr.size() * 8, cudaMemcpyDeviceToHost) != cudaSuccess)
+    return fail(EPS_ERR_CUDA, "build: row offsets download failed");
+  // ---- kNN lists: the rows as queries of the exact scan; with posting lists (IP / cosine), the covered rows'
+  // distances are read from them, bitwise the scan's tile, so the lists do not change ----
+  const bool postings = ix->inv_rows > 0 && (ix->metric == EPS_METRIC_IP || ix->metric == EPS_METRIC_COSINE);
   std::vector<unsigned long long> h_knn(static_cast<size_t>(n) * K);
   {
     DevBuf knn;
     EPS_TRY(knn.reserve(static_cast<size_t>(n) * K * 8));
-    const int64_t qc = 8192;
+    const int64_t qc = 8192;  // queries per scan; with postings, also the rows one plan covers (16 B per element)
     for (int64_t q0 = 0; q0 < n; q0 += qc) {
-      const SparseDist dist(SparseQueries{ix->d_sp_ptr + q0, ix->d_sp_elems, ix->d_sp_norm2 + q0},
-                            std::min(qc, n - q0));
+      const int64_t nq = std::min(qc, n - q0);
+      const SparseDist dist(SparseQueries{ix->d_sp_ptr + q0, ix->d_sp_elems, ix->d_sp_norm2 + q0}, nq);
+      const InvertedDist inv(dist, ptr[q0 + nq] - ptr[q0], ptr[q0]);
       ScanRequest r;
-      r.dist = &dist; r.nq = dist.nq; r.row_end = n; r.k = K; r.metric = ix->metric;
+      r.dist = postings ? static_cast<const DistProducer*>(&inv) : &dist;
+      r.nq = nq; r.row_end = n; r.k = K; r.metric = ix->metric;
       r.skip_deleted = false; r.self_base = q0;
       EPS_TRY(exact_topk(ix, r, knn.as<unsigned long long>() + q0 * K, &st));
     }
@@ -227,14 +234,11 @@ int build_graph_sparse(Index* ix, int64_t n, const eps_build_params* params) {
   // ---- navigation point ----
   int64_t nav = 0;
   {
-    std::vector<int64_t> ptr(static_cast<size_t>(n) + 1);
-    std::vector<uint2> el;
-    cudaError_t e = cudaMemcpy(ptr.data(), ix->d_sp_ptr, ptr.size() * 8, cudaMemcpyDeviceToHost);
-    if (e == cudaSuccess) {
-      el.resize(static_cast<size_t>(ptr[n]));
-      if (!el.empty()) e = cudaMemcpy(el.data(), ix->d_sp_elems, el.size() * 8, cudaMemcpyDeviceToHost);
+    std::vector<uint2> el(static_cast<size_t>(ptr[n]));
+    if (!el.empty()) {
+      const cudaError_t e = cudaMemcpy(el.data(), ix->d_sp_elems, el.size() * 8, cudaMemcpyDeviceToHost);
+      if (e != cudaSuccess) return fail(EPS_ERR_CUDA, cudaGetErrorString(e));
     }
-    if (e != cudaSuccess) return fail(EPS_ERR_CUDA, cudaGetErrorString(e));
     std::unordered_map<uint32_t, float> last;
     for (const uint2& x : el) {
       float v;

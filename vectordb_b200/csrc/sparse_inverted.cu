@@ -21,6 +21,9 @@
 // threads striding over a term's postings (its rows are distinct, so no two threads touch one accumulator), with a
 // barrier after each term that has postings in the slice.  The queries of one slice are adjacent in launch order, so
 // the slice's postings are read from HBM about once and from L2 by the other queries.
+//
+// The sparse graph build (sparse.cu) uses the same producer for its kNN pass: its queries are chunks of the mirror's own
+// rows, whose elements start at the chunk's element offset (InvertedDist::elem_base) rather than at 0.
 #include <cub/cub.cuh>
 
 #include <algorithm>
@@ -99,8 +102,8 @@ __device__ __forceinline__ int64_t rows_lower_bound(const uint2* post, int64_t b
 template <int METRIC>
 __global__ void __launch_bounds__(kInvThreads) inverted_score_kernel(
     const uint2* __restrict__ post, const longlong2* __restrict__ plan, const int64_t* __restrict__ q_ptr,
-    const uint2* __restrict__ q_elems, const float* __restrict__ q_norm2, const float* __restrict__ row_norm2,
-    int64_t nq, int64_t row_start, int64_t n, float* __restrict__ D, int64_t ldd) {
+    const uint2* __restrict__ q_elems, int64_t elem_base, const float* __restrict__ q_norm2,
+    const float* __restrict__ row_norm2, int64_t nq, int64_t row_start, int64_t n, float* __restrict__ D, int64_t ldd) {
   __shared__ float acc[kInvSlice];
   __shared__ int64_t lo_s[kInvThreads], hi_s[kInvThreads];
   __shared__ float qv_s[kInvThreads];
@@ -109,7 +112,8 @@ __global__ void __launch_bounds__(kInvThreads) inverted_score_kernel(
   const int rows = static_cast<int>(min(static_cast<int64_t>(kInvSlice), row_start + n - r0));
   const int32_t row_lo = static_cast<int32_t>(r0), row_hi = static_cast<int32_t>(r0 + rows);
   for (int i = threadIdx.x; i < kInvSlice; i += kInvThreads) acc[i] = 0.f;
-  const int64_t e0 = q_ptr[q], e1 = q_ptr[q + 1];
+  // element offsets relative to the plan's first element (q_elems points at it)
+  const int64_t e0 = q_ptr[q] - elem_base, e1 = q_ptr[q + 1] - elem_base;
   for (int64_t t0 = e0; t0 < e1; t0 += kInvThreads) {
     const int nt = static_cast<int>(min(static_cast<int64_t>(kInvThreads), e1 - t0));
     __syncthreads();  // the accumulators are zeroed and the previous batch's bounds are read
@@ -220,7 +224,7 @@ int InvertedDist::launch(Index* ix, int metric, int64_t row_start, int64_t n, fl
       EPS_TRY(ix->s_inv_plan.reserve(static_cast<size_t>(n_elems) * sizeof(longlong2)));
       if (n_elems > 0) {
         inverted_plan_kernel<<<blocks_for(n_elems, 256), 256, 0, ix->stream>>>(
-            ix->d_inv_terms, ix->inv_terms, ix->d_inv_ptr, scan.q.elems, n_elems, ix->s_inv_plan.as<longlong2>());
+            ix->d_inv_terms, ix->inv_terms, ix->d_inv_ptr, scan.q.elems + elem_base, n_elems, ix->s_inv_plan.as<longlong2>());
         EPS_CUDA(cudaGetLastError());
         ++*launches;
       }
@@ -228,8 +232,9 @@ int InvertedDist::launch(Index* ix, int metric, int64_t row_start, int64_t n, fl
     }
     const auto kernel = metric == EPS_METRIC_IP ? inverted_score_kernel<EPS_METRIC_IP> : inverted_score_kernel<EPS_METRIC_COSINE>;
     kernel<<<static_cast<unsigned>(blocks), kInvThreads, 0, ix->stream>>>(ix->d_inv_post, ix->s_inv_plan.as<longlong2>(),
-                                                                         scan.q.ptr, scan.q.elems, scan.q.norm2,
-                                                                         ix->d_sp_norm2, nq, row_start, covered, D, ldd);
+                                                                         scan.q.ptr, scan.q.elems + elem_base, elem_base,
+                                                                         scan.q.norm2, ix->d_sp_norm2, nq, row_start,
+                                                                         covered, D, ldd);
     EPS_CUDA(cudaGetLastError());
     ++*launches;
   }

@@ -419,6 +419,34 @@ EPS_API int eps_index_build_sparse_inverted(eps_index* ix, int64_t n);
  * EPS_ERR_INVALID_ARGUMENT. */
 EPS_API int eps_index_sparse_inverted_info(eps_index* ix, int64_t* n_rows, int64_t* n_terms, int64_t* n_postings);
 
+/* L2 screen of a sparse L2 index: the posting lists of rows [0, n), with the same arrays, layout and build as
+ * eps_index_build_sparse_inverted (whose info reports their rows, terms and postings on an L2 index too).
+ * What it does to results: nothing; it is not a search mode.  Every exact sparse scan a search call runs (the places
+ * listed for the inverted index) and the kNN pass of eps_index_build give each covered row a proven lower bound LB of
+ * the reference's L2 distance D_ref from the postings, and compute D_ref itself (the merge of the scan) only for rows
+ * that can still be among the K best: per chunk of rows, the K rows with the smallest bounds are re-scored, T = the
+ * largest of their distances, and every row with LB <= T is re-scored; the others cannot beat those K rows.  Ids,
+ * counts, bitwise distances and the n_dist / n_seed / n_expand / n_edges counters are what they are without the screen,
+ * and eps_index_build installs the same graph.  Only kernel_launches and the timings change.  A search whose filter
+ * compares "@distance" (outside prefilter mode) takes the merge for every row and re-scores nothing.
+ * The bound: with m_r and m_q the row's and the query's element counts, m = m_r + m_q, u = 2^-24,
+ * gamma_k = k u / (1 - k u), D the real distance, every term the reference adds is non-negative, so when nothing
+ * overflows |D_ref - D| <= gamma_{m+2} D + m 2^-149 (the second term covers products that underflow).  D is bounded
+ * below from the posting lists' fp32 dot of the matched elements, the stored fp32 |row|^2, the query's fp32 |q|^2
+ * (each a sequential sum with a known error bound) and m_r, every step rounded toward -inf (sparse_inverted.cu
+ * restates the derivation).  Rows with a non-finite |row|^2 (NaN or +-inf values, squares that overflow), pairs with
+ * m + 2 > 2^20, and every row for a query with a non-finite |q|^2 are always re-scored.
+ * Lifecycle as for the inverted index: rows appended after the build are merged until the next build; n = 0 drops the
+ * lists; a refused or failed call leaves the previous state; views created after the build share it.  Refusals, all
+ * EPS_ERR_INVALID_ARGUMENT: a null or dense index, an inner-product or cosine index (eps_index_build_sparse_inverted
+ * gives those exact distances from the same lists), n < 0, n above the mirrored rows, a view, or an index with live
+ * views.  Device memory: as for the inverted index, plus 8 B x nq x k (x the scan's row splits) for the K best keys. */
+EPS_API int eps_index_build_sparse_l2_screen(eps_index* ix, int64_t n);
+/* Rows the L2 screen covers (0 = none, and 0 on an inner-product or cosine index) and the (query, row) pairs this
+ * handle's searches and builds have re-scored through the merge so far; waits for the index's stream.  Any pointer may
+ * be NULL.  A null or dense index: EPS_ERR_INVALID_ARGUMENT. */
+EPS_API int eps_index_sparse_l2_screen_info(eps_index* ix, int64_t* n_rows, uint64_t* n_rescored);
+
 /* Raw stream handle (cudaStream_t) the index launches on, for callers that time with CUDA events. */
 EPS_API void* eps_index_stream(eps_index* ix);
 

@@ -567,11 +567,38 @@ static int fp32_scan(Index* ix, const ScanRequest& r, unsigned long long* d_topk
   a.D = s.D; a.ldd = s.chunk; a.nsplit = nsplit; a.k = static_cast<int>(k); a.state = state;
   a.pass = s.pass; a.pass_base = r.row_start; a.self_base = r.self_base;
   if (filter_reads_distance(r)) { a.dyn = r.d_prog; a.attrs = ix->d_attrs; a.attr_stride = ix->attr_stride; }
+  // The L2 screen (SparseL2Screen, sparse_inverted.cu) selects K = k keys of the bound tile first, into its own lists
+  // [nq x nsplit x k] (then merged into [nq x k]), followed by T [nq].  A filter that reads the distance would select
+  // them by bounds: such a call takes the merge tile for every row.
+  const SparseL2Screen* screen = filter_reads_distance(r) ? nullptr : r.l2_screen;
+  SelectArgs b = a, bm;
+  unsigned long long* b_merged = nullptr;
+  float* T = nullptr;
+  if (screen) {
+    const size_t lists = static_cast<size_t>(nq) * nsplit * k, merged = nsplit > 1 ? static_cast<size_t>(nq) * k : 0;
+    EPS_TRY(ix->s_l2_screen.reserve((lists + merged) * 8 + static_cast<size_t>(nq) * 4));
+    b.state = ix->s_l2_screen.as<unsigned long long>();
+    b_merged = nsplit > 1 ? b.state + lists : b.state;
+    T = reinterpret_cast<float*>(b.state + lists + merged);
+    bm.keys_in = b.state; bm.n = static_cast<int64_t>(nsplit) * k; bm.k = static_cast<int>(k); bm.state = b_merged;
+  }
   for (int64_t c0 = 0; c0 < n; c0 += s.chunk) {
     a.row_base = r.row_start + c0;
     a.n = std::min(s.chunk, n - c0);
-    if (r.dist) EPS_TRY(r.dist->launch(ix, r.metric, a.row_base, a.n, s.D, s.chunk, &launches));
-    else EPS_TRY(launch_distances(ix, r.metric, ix->d_vectors, a.row_base, a.n, r.queries, nq, s.D, s.chunk, &launches));
+    if (screen) {
+      EPS_TRY(screen->bounds(ix, a.row_base, a.n, s.D, s.chunk, &launches));
+      b.row_base = a.row_base; b.n = a.n;
+      fill_inf(ix, b.state, nq * nsplit * k, &launches);
+      if (nsplit > 1) fill_inf(ix, b_merged, nq * k, &launches);
+      EPS_TRY(run_select<false>(ix, b, nq, s.smem, &launches));
+      if (nsplit > 1) EPS_TRY(run_select<true>(ix, bm, nq, s.smem, &launches));
+      EPS_TRY(screen->threshold(ix, b_merged, static_cast<int>(k), T, &launches));
+      EPS_TRY(screen->rescore(ix, a.row_base, a.n, s.D, s.chunk, T, s.pass, r.row_start, r.self_base, &launches));
+    } else if (r.dist) {
+      EPS_TRY(r.dist->launch(ix, r.metric, a.row_base, a.n, s.D, s.chunk, &launches));
+    } else {
+      EPS_TRY(launch_distances(ix, r.metric, ix->d_vectors, a.row_base, a.n, r.queries, nq, s.D, s.chunk, &launches));
+    }
     EPS_TRY(run_select<false>(ix, a, nq, s.smem, &launches));
   }
   if (nsplit > 1) {

@@ -246,8 +246,13 @@ struct DenseBatch : QueryBatch {
 
 struct SparseBatch : QueryBatch {
   const SparseDist& dist;  // the caller's: a copy of the batch still points at it
-  // tile: the exact scan's producer, d itself or the inverted index's (the graph search always takes the raw queries)
-  SparseBatch(const SparseDist& d, const DistProducer& tile) : dist(d) { scan.dist = &tile; scan.nq = d.nq; }
+  // tile: the exact scan's producer, d itself or the inverted index's (the graph search always takes the raw queries);
+  // l2_screen: the L2 screen's, or null
+  SparseBatch(const SparseDist& d, const DistProducer& tile, const SparseL2Screen* l2_screen) : dist(d) {
+    scan.dist = &tile;
+    scan.nq = d.nq;
+    scan.l2_screen = l2_screen;
+  }
   int graph(Index* ix, int64_t L, unsigned long long* d_queue, eps_stats* st) const override {
     return sparse_graph_search(ix, dist.q, dist.nq, L, d_queue, st);
   }
@@ -812,9 +817,12 @@ int eps_search_sparse_batch(eps_index* h, int64_t nq, const int64_t* q_offsets, 
   EPS_TRY(eps::upload_sparse_queries(ix, qp, qe, qn, &ix->s_sparse_q, &q));
   const eps::SparseDist dist(q, nq);
   const eps::InvertedDist inv(dist, static_cast<int64_t>(qe.size()));
-  const eps::DistProducer& tile = ix->inv_rows > 0 ? static_cast<const eps::DistProducer&>(inv) : dist;
-  return eps::search_to_host(ix, eps::SparseBatch(dist, tile), nq, limit, filter, n_filter, out_ids, out_dists,
-                             out_counts, stats);
+  const eps::SparseL2Screen screen(inv);
+  // posting lists: the inverted index of an IP / cosine index, the L2 screen of an L2 one
+  const bool lists = ix->inv_rows > 0, l2 = ix->metric == EPS_METRIC_L2;
+  const eps::DistProducer& tile = lists && !l2 ? static_cast<const eps::DistProducer&>(inv) : dist;
+  return eps::search_to_host(ix, eps::SparseBatch(dist, tile, lists && l2 ? &screen : nullptr), nq, limit, filter,
+                             n_filter, out_ids, out_dists, out_counts, stats);
 }
 
 int eps_index_build_sparse_inverted(eps_index* h, int64_t n) {
@@ -823,7 +831,8 @@ int eps_index_build_sparse_inverted(eps_index* h, int64_t n) {
   if (!ix->sparse) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "inverted index on a dense index");
   if (ix->metric == EPS_METRIC_L2)
     return eps::fail(EPS_ERR_UNSUPPORTED, "inverted index on an L2 index: the L2 sum also adds the row-only and "
-                                          "query-only terms in merged index order, which posting lists cannot reproduce");
+                                          "query-only terms in merged index order, which posting lists cannot reproduce "
+                                          "(eps_index_build_sparse_l2_screen builds the L2 screen)");
   EPS_TRY(check_mutable(ix));
   if (n < 0 || n > ix->n_rows) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "inverted index: n outside [0, mirrored rows]");
   EPS_TRY(eps::check_device(ix->device));
@@ -837,6 +846,37 @@ int eps_index_sparse_inverted_info(eps_index* h, int64_t* n_rows, int64_t* n_ter
   if (n_rows) *n_rows = ix->inv_rows;
   if (n_terms) *n_terms = ix->inv_terms;
   if (n_postings) *n_postings = ix->inv_postings;
+  return EPS_OK;
+}
+
+int eps_index_build_sparse_l2_screen(eps_index* h, int64_t n) {
+  Index* ix = reinterpret_cast<Index*>(h);
+  if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");
+  if (!ix->sparse) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "L2 screen on a dense index");
+  if (ix->metric != EPS_METRIC_L2)
+    return eps::fail(EPS_ERR_INVALID_ARGUMENT, "L2 screen on an inner-product or cosine index: its posting lists give "
+                                               "the exact distances (eps_index_build_sparse_inverted)");
+  EPS_TRY(check_mutable(ix));
+  if (n < 0 || n > ix->n_rows) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "L2 screen: n outside [0, mirrored rows]");
+  EPS_TRY(eps::check_device(ix->device));
+  return eps::build_sparse_inverted(ix, n);
+}
+
+int eps_index_sparse_l2_screen_info(eps_index* h, int64_t* n_rows, uint64_t* n_rescored) {
+  Index* ix = reinterpret_cast<Index*>(h);
+  if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");
+  if (!ix->sparse) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "L2 screen info on a dense index");
+  if (n_rows) *n_rows = ix->metric == EPS_METRIC_L2 ? ix->inv_rows : 0;
+  if (n_rescored) {
+    *n_rescored = 0;
+    if (ix->d_l2_rescored) {
+      EPS_TRY(eps::check_device(ix->device));
+      EPS_CUDA(cudaStreamSynchronize(ix->stream));
+      unsigned long long v = 0;
+      EPS_CUDA(cudaMemcpy(&v, ix->d_l2_rescored, 8, cudaMemcpyDeviceToHost));
+      *n_rescored = v;
+    }
+  }
   return EPS_OK;
 }
 

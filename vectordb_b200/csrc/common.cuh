@@ -172,6 +172,20 @@ __device__ __forceinline__ float sparse_finish(float acc, float rn, float qn) {
   return d;
 }
 
+// Distance of table row `id` (CSR row_ptr / elems, fp32 |row|^2 in row_norm2) to the query q[0 .. n), one thread,
+// through SparseMerge and sparse_finish: the sparse graph search and the L2 screen's re-score (sparse_inverted.cu).
+template <int METRIC>
+__device__ __forceinline__ float sparse_row_dist(const int64_t* row_ptr, const uint2* elems, const float* row_norm2,
+                                                 uint32_t id, const uint2* q, int64_t n, float qn) {
+  const int64_t p0 = row_ptr[id], p1 = row_ptr[id + 1];
+  SparseMerge<METRIC> mg(q, 0, n);
+  for (int64_t c = p0; c < p1; ++c) {
+    const uint2 e = __ldg(elems + c);
+    mg.add(e.x, __uint_as_float(e.y));
+  }
+  return sparse_finish<METRIC>(mg.sum(), METRIC == EPS_METRIC_COSINE ? row_norm2[id] : 0.f, qn);
+}
+
 // Per-lane partial of one row against the query held in shared memory.
 // VEC4 path: dim % 4 == 0 and 16-byte aligned rows; lane l covers float4 chunks l, l+32, ...
 template <bool L2>

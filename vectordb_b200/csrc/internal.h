@@ -87,7 +87,8 @@ struct Table {
   DevArray<uint2> d_sp_elems;   // {index, value bits}, indices strictly increasing within a row
   DevArray<float> d_sp_norm2;   // [rows] sequential fp32 sum of squares of each row (cosine); its room is the row room
   int64_t sp_nnz = 0;
-  // inverted index of the sparse rows [0, inv_rows) (sparse_inverted.cu): the exact scan reads their distances from it
+  // posting lists of the sparse rows [0, inv_rows) (sparse_inverted.cu): the exact scan reads their distances from them
+  // (IP / cosine: the inverted index), or screens them with a lower bound of their distance (L2: the L2 screen)
   DevArray<uint32_t> d_inv_terms;  // [inv_terms] the distinct indices, ascending
   DevArray<int64_t> d_inv_ptr;     // [inv_terms + 1] posting offsets of the terms
   DevArray<uint2> d_inv_post;      // [inv_postings] {int32 row, float value bits}, rows ascending within a term
@@ -168,7 +169,7 @@ struct Index : Table, Config {
   // scratch
   DevBuf s_queries, s_dist, s_topk, s_topk2, s_pass, s_filter, s_vset, s_visited, s_vlog, s_queue, s_tail, s_out_ids, s_out_dists,
       s_out_counts, s_stats, s_misc, s_seed_rows, s_seed_dist, s_xnorm, s_qnorm, s_coarse, s_thr, s_cand, s_cand_cnt, s_bf16, s_qbf16, s_flags,
-      s_sparse_q, s_xnorm_max, s_like, s_like_jobs, s_inv_plan;
+      s_sparse_q, s_xnorm_max, s_like, s_like_jobs, s_inv_plan, s_l2_screen;
   int64_t bf16_rows = 0;         // rows converted into s_bf16 while it had generation bf16_gen
   uint64_t bf16_gen = 0;
   int64_t xnorm_rows = 0;        // rows whose |x|^2 is current in s_xnorm; s_xnorm_max holds the largest (float bits)
@@ -183,10 +184,12 @@ struct Index : Table, Config {
   bool prof_timeline = false;    // developer build: s_prof_qtimes belongs to the last launch
   DevBuf s_qsk;                  // [nq x sk_m] query sketches, then [nq] their error bounds
   DevArray<unsigned long long> d_screened;  // device count of the fresh neighbours the screen dropped on this handle
+  DevArray<unsigned long long> d_l2_rescored;  // device count of the (query, row) pairs the L2 screen re-scored here
   HostBuf h_out;                 // pinned host mirror of the packed result block (eps_search_batch)
 };
 
 // ---- brute_force.cu ------------------------------------------------------------------------
+struct SparseL2Screen;
 // Producer of the [nq x ldd] fp32 distance tile of rows [row_start, row_start + n) that the exact scan selects from,
 // in place of launch_distances (the sparse scan, sparse.cu).
 struct DistProducer {
@@ -205,6 +208,9 @@ struct ScanRequest {
   bool prefilter = false;              // evaluate the filter with distance 0
   bool skip_deleted = true;            // false: the build indexes every row, deleted or not (ann_graph_segment.cpp:201)
   int64_t self_base = -1;              // >= 0: row self_base + q is left out of query q's list (the build's kNN lists)
+  // sparse L2 index with posting lists: fp32_scan bounds, thresholds and re-scores the covered rows before the select
+  // (dist is then the plain SparseDist: a filter that reads the distance takes it for every row)
+  const SparseL2Screen* l2_screen = nullptr;
 };
 // Exact top-k of rows [row_start, row_end): per-query sorted keys (make_key(dist,row)) in d_topk [nq x k], kKeyInf
 // padded.
@@ -255,7 +261,7 @@ int sparse_append(Index* ix, int64_t first_row, int64_t n_rows, const int64_t* o
 int build_graph_sparse(Index* ix, int64_t n, const eps_build_params* params);
 
 // ---- sparse_inverted.cu --------------------------------------------------------------------
-// Posting lists of rows [0, n) of a sparse IP / cosine index (n = 0 drops them); the caller has validated ix and n.
+// Posting lists of rows [0, n) of a sparse index (n = 0 drops them); the caller has validated ix and n.
 int build_sparse_inverted(Index* ix, int64_t n);
 // The sparse scan's distance tile with the rows [0, inv_rows) read from the posting lists, bitwise the tile of
 // SparseDist: each row's products are added in the query's index order, from 0, as sparse_dist_kernel adds them.
@@ -269,6 +275,27 @@ struct InvertedDist : DistProducer {
   InvertedDist(const SparseDist& s, int64_t n_elems_, int64_t elem_base_ = 0)
       : scan(s), n_elems(n_elems_), elem_base(elem_base_) {}
   int launch(Index* ix, int metric, int64_t row_start, int64_t n, float* D, int64_t ldd, uint64_t* launches) const override;
+  int plan(Index* ix, uint64_t* launches) const;  // once per call, before the first score launch
+};
+// The L2 screen (eps_index_build_sparse_l2_screen): the posting lists of an L2 index give each covered row a proven
+// lower bound LB <= D_ref of the reference's distance; fp32_scan (brute_force.cu) runs, per chunk of rows,
+//   1. bounds():    the tile with LB for the covered rows (+inf for rows the bound does not cover) and the exact
+//                   distances of the others (SparseDist);
+//   2. the select of each query's K smallest tile keys (K = the scan's k), then threshold(): T[q] = the largest exact
+//                   distance of those K rows (+inf when fewer than K finite keys came back or one is NaN);
+//   3. rescore():   the exact distance of every covered row with LB <= T[q] or not covered by the bound, +inf for the
+//                   others (the K rows of step 2 have D_ref <= T, so a row with LB > T is not among the K best);
+//   4. the unchanged select over the tile.
+struct SparseL2Screen {
+  InvertedDist inv;
+  explicit SparseL2Screen(const InvertedDist& i) : inv(i) {}
+  int bounds(Index* ix, int64_t row_start, int64_t n, float* D, int64_t ldd, uint64_t* launches) const;
+  // keys: [nq x k] sorted keys of the tile of step 1; T: [nq]
+  int threshold(Index* ix, const unsigned long long* keys, int k, float* T, uint64_t* launches) const;
+  // the covered rows of [row_start, row_start + n); pass (relative to pass_base, may be null) and self_base as in the
+  // select: rows it drops are not re-scored
+  int rescore(Index* ix, int64_t row_start, int64_t n, float* D, int64_t ldd, const float* T, const uint32_t* pass,
+              int64_t pass_base, int64_t self_base, uint64_t* launches) const;
 };
 
 // ---- sparse_graph.cu -----------------------------------------------------------------------

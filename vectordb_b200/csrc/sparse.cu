@@ -209,9 +209,10 @@ int build_graph_sparse(Index* ix, int64_t n, const eps_build_params* params) {
   std::vector<int64_t> ptr(static_cast<size_t>(n) + 1);  // the rows' element offsets (ptr[0] = 0)
   if (cudaMemcpy(ptr.data(), ix->d_sp_ptr, ptr.size() * 8, cudaMemcpyDeviceToHost) != cudaSuccess)
     return fail(EPS_ERR_CUDA, "build: row offsets download failed");
-  // ---- kNN lists: the rows as queries of the exact scan; with posting lists (IP / cosine), the covered rows'
-  // distances are read from them, bitwise the scan's tile, so the lists do not change ----
-  const bool postings = ix->inv_rows > 0 && (ix->metric == EPS_METRIC_IP || ix->metric == EPS_METRIC_COSINE);
+  // ---- kNN lists: the rows as queries of the exact scan; with posting lists, the covered rows' distances are read
+  // from them (IP / cosine: bitwise the scan's tile) or screened and re-scored (L2: the same K best), so the lists do
+  // not change ----
+  const bool postings = ix->inv_rows > 0, l2 = ix->metric == EPS_METRIC_L2;
   std::vector<unsigned long long> h_knn(static_cast<size_t>(n) * K);
   {
     DevBuf knn;
@@ -221,8 +222,10 @@ int build_graph_sparse(Index* ix, int64_t n, const eps_build_params* params) {
       const int64_t nq = std::min(qc, n - q0);
       const SparseDist dist(SparseQueries{ix->d_sp_ptr + q0, ix->d_sp_elems, ix->d_sp_norm2 + q0}, nq);
       const InvertedDist inv(dist, ptr[q0 + nq] - ptr[q0], ptr[q0]);
+      const SparseL2Screen screen(inv);
       ScanRequest r;
-      r.dist = postings ? static_cast<const DistProducer*>(&inv) : &dist;
+      r.dist = postings && !l2 ? static_cast<const DistProducer*>(&inv) : &dist;
+      if (postings && l2) r.l2_screen = &screen;
       r.nq = nq; r.row_end = n; r.k = K; r.metric = ix->metric;
       r.skip_deleted = false; r.self_base = q0;
       EPS_TRY(exact_topk(ix, r, knn.as<unsigned long long>() + q0 * K, &st));

@@ -54,18 +54,6 @@ struct SGArgs {
   int L, Lp, nq;
 };
 
-// Distance of table row `id` to the query q[0 .. n), through the scan's SparseMerge and sparse_finish.
-template <int METRIC>
-__device__ __forceinline__ float sparse_row_dist(const SGArgs& a, uint32_t id, const uint2* q, int64_t n, float qn) {
-  const int64_t p0 = a.row_ptr[id], p1 = a.row_ptr[id + 1];
-  SparseMerge<METRIC> mg(q, 0, n);
-  for (int64_t c = p0; c < p1; ++c) {
-    const uint2 e = __ldg(a.elems + c);
-    mg.add(e.x, __uint_as_float(e.y));
-  }
-  return sparse_finish<METRIC>(mg.sum(), METRIC == EPS_METRIC_COSINE ? a.row_norm2[id] : 0.f, qn);
-}
-
 // Test-and-insert of one id into the hash set: one 32-byte bucket read; an entry equal to the id = visited; else a CAS
 // on the first free entry of the bucket (the next bucket's first entry when it is full), and a CAS lost to another id
 // goes on probing entry by entry (the dense kernel's step, one id per thread).  True when this thread inserted it.
@@ -131,7 +119,7 @@ __global__ void __launch_bounds__(kGsThreads) sparse_graph_search_kernel(SGArgs 
         const uint32_t id = static_cast<uint32_t>(a.init_ids[i]);
         if (hashed) vset_claim(vset, vmask, vset_bucket(id, a.vset_shift), id, vacc);
         else atomicOr(&visited[id >> 5], 1u << (id & 31));
-        key = make_key(sparse_row_dist<METRIC>(a, id, qv, qn_el, qn), id);
+        key = make_key(sparse_row_dist<METRIC>(a.row_ptr, a.elems, a.row_norm2, id, qv, qn_el, qn), id);
       }
       qa[i] = key;
     }
@@ -224,7 +212,8 @@ __global__ void __launch_bounds__(kGsThreads) sparse_graph_search_kernel(SGArgs 
         // distances, one fresh row per thread; dist > worst-in-queue is rejected (:424), ties by id
         if (tid < total) {
           const uint32_t id = static_cast<uint32_t>(fresh[tid]);
-          const unsigned long long key = make_key(sparse_row_dist<METRIC>(a, id, qv, qn_el, qn), id);
+          const float d = sparse_row_dist<METRIC>(a.row_ptr, a.elems, a.row_norm2, id, qv, qn_el, qn);
+          const unsigned long long key = make_key(d, id);
           if (key < (qa[L - 1] & kKeyMask)) pend[atomicAdd(&s_npend, 1)] = key;
         }
         n_fresh += static_cast<uint32_t>(total);

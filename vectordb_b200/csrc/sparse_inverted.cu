@@ -1,13 +1,17 @@
-// Inverted index of a sparse IP / cosine field (eps_index_build_sparse_inverted, DESIGN.md §K5): per-term posting lists
-// of rows [0, inv_rows), from which the exact scan's distance tile is computed instead of merging every (query, row)
-// pair.
+// Posting lists of a sparse field (DESIGN.md §K5): per-term posting lists of rows [0, inv_rows).  On an IP / cosine
+// field they are the inverted index (eps_index_build_sparse_inverted): the exact scan's distance tile is computed from
+// them instead of merging every (query, row) pair.  On an L2 field they are the L2 screen
+// (eps_index_build_sparse_l2_screen): the same score kernel writes a proven lower bound of each covered row's distance
+// (sparse_l2_lower_bound), and only the rows whose bound can still place them among the k best are merged
+// (l2_threshold_kernel, l2_rescore_kernel; the steps are driven by fp32_scan, brute_force.cu).
 //
 // Why the tile is bitwise the scan's: for IP and cosine the reference adds the matched products row[i] * query[i] in
 // increasing index order, from 0 (engine/db/vector.cpp:7-47).  inverted_score_kernel walks a query's elements in their
 // (increasing) index order and adds each term's posting value times the query value into a per-row fp32 accumulator
 // that starts at 0, with __fmul_rn / __fadd_rn: every row sees the same operations in the same order as in SparseMerge
 // (common.cuh), and the tile finishes through sparse_finish like every other sparse distance.  A row that matches
-// nothing keeps 0, as in the merge.  L2 cannot be served: its merged order also adds the row-only and query-only terms.
+// nothing keeps 0, as in the merge.  L2 cannot be served that way: its merged order also adds the row-only and
+// query-only terms; the screen bounds it instead and takes the exact value from SparseMerge.
 //
 // Build: expand the CSR elements of rows [0, n) to (index, {row, value}) pairs, sort them by index with a stable radix
 // sort (rows stay ascending within a term), flag the first posting of each term and take the int64 exclusive sum of the
@@ -99,11 +103,42 @@ __device__ __forceinline__ int64_t rows_lower_bound(const uint2* post, int64_t b
   return b;
 }
 
+// Lower bound of the reference's L2 distance D_ref of a (row, query) pair from the fp32 dot of their matched elements
+// (the score kernel's accumulator), the fp32 squared norms rn = d_sp_norm2[row] and qn, and the element counts m_r and
+// m_q; +inf when the bound does not cover the pair.  Derivation (u = 2^-24, eta = 2^-149, gamma_k = k u / (1 - k u),
+// m = m_r + m_q, R2 / Q2 / P the real |row|^2, |query|^2 and <row, query>, D = R2 + Q2 - 2 P):
+//   * rn is a sequential sum of m_r non-negative fl(v * v): |rn - R2| <= gamma_{m_r} R2 + m_r eta (a product that
+//     underflows is off by at most 2^-150; a sum with a subnormal result is exact), so
+//     R2 >= max(0, (1 - gamma_{m_r}) (rn - m_r eta)); the same for Q2 with qn and m_q;
+//   * dot sums c <= m products fl(r_i q_i): |dot - P| <= gamma_m sum |r_i q_i| + m eta, and sum |r_i q_i| <= (R2 + Q2) / 2,
+//     so D >= (1 - gamma_m) (R2 + Q2) - 2 dot - 2 m eta, and D >= 0;
+//   * D_ref adds m' <= m non-negative terms fl(fl(a - b)^2) or fl(v * v), each within m + 2 roundings of its real value:
+//     D_ref >= (1 - gamma_{m+2}) D - m eta (when D_ref is finite; +inf bounds itself).
+// Every step is rounded toward -inf in fp64.  m + 2 <= 2^20 keeps k u <= 2^-4, where gamma_k <= (9/8) k u and
+// 1 - (9/8) k u is exact.  Pairs with a non-finite input or more elements get +inf: they are always re-scored.
+constexpr int64_t kL2BoundTerms = 1 << 20;
+
+__device__ __forceinline__ float sparse_l2_lower_bound(float dot, float rn, float qn, int64_t m_r, int64_t m_q) {
+  const int64_t m = m_r + m_q;
+  if (!isfinite(dot) || !isfinite(rn) || !isfinite(qn) || m + 2 > kL2BoundTerms) return INFINITY;
+  const double eta = 0x1p-149;
+  const auto one_minus_gamma = [](int64_t k) { return 1.0 - static_cast<double>(k) * (1.125 * 0x1p-24); };  // exact
+  // k * eta and 2 * dot are exact in fp64
+  const double r2 = fmax(0.0, __dmul_rd(one_minus_gamma(m_r), __dadd_rd(rn, -static_cast<double>(m_r) * eta)));
+  const double q2 = fmax(0.0, __dmul_rd(one_minus_gamma(m_q), __dadd_rd(qn, -static_cast<double>(m_q) * eta)));
+  double d = __dmul_rd(one_minus_gamma(m), __dadd_rd(r2, q2));
+  d = __dadd_rd(__dadd_rd(d, -2.0 * static_cast<double>(dot)), -2.0 * static_cast<double>(m) * eta);
+  const double lb = __dadd_rd(__dmul_rd(one_minus_gamma(m + 2), fmax(d, 0.0)), -static_cast<double>(m) * eta);
+  return __double2float_rd(lb);
+}
+
+// IP / cosine: the distance tile.  L2: the lower-bound tile of the L2 screen (row_ptr gives each row's element count).
 template <int METRIC>
 __global__ void __launch_bounds__(kInvThreads) inverted_score_kernel(
     const uint2* __restrict__ post, const longlong2* __restrict__ plan, const int64_t* __restrict__ q_ptr,
     const uint2* __restrict__ q_elems, int64_t elem_base, const float* __restrict__ q_norm2,
-    const float* __restrict__ row_norm2, int64_t nq, int64_t row_start, int64_t n, float* __restrict__ D, int64_t ldd) {
+    const float* __restrict__ row_norm2, const int64_t* __restrict__ row_ptr, int64_t nq, int64_t row_start, int64_t n,
+    float* __restrict__ D, int64_t ldd) {
   __shared__ float acc[kInvSlice];
   __shared__ int64_t lo_s[kInvThreads], hi_s[kInvThreads];
   __shared__ float qv_s[kInvThreads];
@@ -139,13 +174,91 @@ __global__ void __launch_bounds__(kInvThreads) inverted_score_kernel(
   }
   __syncthreads();
   float qn = 0.f;
-  if (METRIC == EPS_METRIC_COSINE) qn = q_norm2[q];
+  if (METRIC != EPS_METRIC_IP) qn = q_norm2[q];
   float* out = D + q * ldd + (r0 - row_start);
   for (int i = threadIdx.x; i < rows; i += kInvThreads) {
     float rn = 0.f;
-    if (METRIC == EPS_METRIC_COSINE) rn = row_norm2[r0 + i];
-    out[i] = sparse_finish<METRIC>(acc[i], rn, qn);
+    if (METRIC != EPS_METRIC_IP) rn = row_norm2[r0 + i];
+    if (METRIC == EPS_METRIC_L2)
+      out[i] = sparse_l2_lower_bound(acc[i], rn, qn, row_ptr[r0 + i + 1] - row_ptr[r0 + i], e1 - e0);
+    else
+      out[i] = sparse_finish<METRIC>(acc[i], rn, qn);
   }
+}
+
+// Step 2 of the L2 screen: T[q] = the largest exact distance of the K rows of keys[q] (+inf when one is missing, has an
+// unbounded key or a NaN distance).  Rows at or above inv_rows carry their exact distance in the key already.
+constexpr int kL2Threads = 256;
+__global__ void __launch_bounds__(kL2Threads) l2_threshold_kernel(
+    const int64_t* __restrict__ row_ptr, const uint2* __restrict__ elems, int64_t inv_rows, const int64_t* __restrict__ q_ptr,
+    const uint2* __restrict__ q_elems, const unsigned long long* __restrict__ keys, int k, float* __restrict__ T,
+    unsigned long long* __restrict__ n_rescored) {
+  __shared__ unsigned t_bits;  // exact distances are >= +0 and order as their bits
+  __shared__ unsigned long long cnt;
+  const int64_t q = blockIdx.x;
+  if (threadIdx.x == 0) { t_bits = 0u; cnt = 0ull; }
+  __syncthreads();
+  const uint2* qv = q_elems + q_ptr[q];
+  const int64_t qn_el = q_ptr[q + 1] - q_ptr[q];
+  unsigned my = 0u, mine = 0u;
+  for (int j = threadIdx.x; j < k; j += kL2Threads) {
+    const unsigned long long key = keys[q * k + j] & kKeyMask;
+    float d = key_dist(key);
+    if (key == kKeyInf || isinf(d)) {
+      d = INFINITY;
+    } else if (key_id(key) < inv_rows) {
+      d = sparse_row_dist<EPS_METRIC_L2>(row_ptr, elems, nullptr, key_id(key), qv, qn_el, 0.f);
+      ++mine;
+    }
+    if (d != d) d = INFINITY;
+    my = max(my, __float_as_uint(d));
+  }
+  atomicMax(&t_bits, my);
+  if (mine) atomicAdd(&cnt, static_cast<unsigned long long>(mine));
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    T[q] = __uint_as_float(t_bits);
+    if (cnt) atomicAdd(n_rescored, cnt);
+  }
+}
+
+// Step 3: one CTA = one query x kInvSlice rows of the tile.  A row the select will keep (pass bit set, not the query's
+// own row) whose bound is <= T[q] or +inf gets its exact distance; every other row gets +inf.
+__global__ void __launch_bounds__(kL2Threads) l2_rescore_kernel(
+    const int64_t* __restrict__ row_ptr, const uint2* __restrict__ elems, const int64_t* __restrict__ q_ptr,
+    const uint2* __restrict__ q_elems, const float* __restrict__ T, const uint32_t* __restrict__ pass, int64_t pass_base,
+    int64_t self_base, int64_t nq, int64_t row_start, int64_t n, float* __restrict__ D, int64_t ldd,
+    unsigned long long* __restrict__ n_rescored) {
+  __shared__ unsigned cnt;
+  const int64_t q = blockIdx.x % nq, s = blockIdx.x / nq;
+  const int64_t i0 = s * kInvSlice;
+  const int rows = static_cast<int>(min(static_cast<int64_t>(kInvSlice), n - i0));
+  if (threadIdx.x == 0) cnt = 0u;
+  __syncthreads();
+  const float t = T[q];
+  const uint2* qv = q_elems + q_ptr[q];
+  const int64_t qn_el = q_ptr[q + 1] - q_ptr[q];
+  float* out = D + q * ldd + i0;
+  unsigned mine = 0u;
+  for (int i = threadIdx.x; i < rows; i += kL2Threads) {
+    const int64_t r = row_start + i0 + i;
+    const float lb = out[i];
+    bool ok = lb <= t || lb == INFINITY;
+    if (ok && pass) {
+      const int64_t pi = r - pass_base;
+      ok = (pass[pi >> 5] >> (pi & 31)) & 1u;
+    }
+    if (ok && self_base >= 0 && r == self_base + q) ok = false;
+    float d = INFINITY;
+    if (ok) {
+      d = sparse_row_dist<EPS_METRIC_L2>(row_ptr, elems, nullptr, static_cast<uint32_t>(r), qv, qn_el, 0.f);
+      ++mine;
+    }
+    out[i] = d;
+  }
+  if (mine) atomicAdd(&cnt, mine);
+  __syncthreads();
+  if (threadIdx.x == 0 && cnt) atomicAdd(n_rescored, static_cast<unsigned long long>(cnt));
 }
 
 unsigned blocks_for(int64_t threads, int per_block) { return static_cast<unsigned>((threads + per_block - 1) / per_block); }
@@ -210,35 +323,113 @@ int build_sparse_inverted(Index* ix, int64_t n) {
   return EPS_OK;
 }
 
-int InvertedDist::launch(Index* ix, int metric, int64_t row_start, int64_t n, float* D, int64_t ldd,
-                         uint64_t* launches) const {
-  if (n <= 0 || scan.nq <= 0) return EPS_OK;
-  const int64_t nq = scan.nq;
-  const int64_t covered = std::max<int64_t>(0, std::min(row_start + n, ix->inv_rows) - row_start);
-  if (covered > 0) {
-    if (metric != EPS_METRIC_IP && metric != EPS_METRIC_COSINE)
-      return fail(EPS_ERR_UNSUPPORTED, "inverted index: only inner-product and cosine distances are read from postings");
-    const int64_t blocks = nq * ((covered + kInvSlice - 1) / kInvSlice);
-    if (blocks > 0x7fffffffll) return fail(EPS_ERR_UNSUPPORTED, "inverted index: too many queries in one launch");
-    if (!planned) {
-      EPS_TRY(ix->s_inv_plan.reserve(static_cast<size_t>(n_elems) * sizeof(longlong2)));
-      if (n_elems > 0) {
-        inverted_plan_kernel<<<blocks_for(n_elems, 256), 256, 0, ix->stream>>>(
-            ix->d_inv_terms, ix->inv_terms, ix->d_inv_ptr, scan.q.elems + elem_base, n_elems, ix->s_inv_plan.as<longlong2>());
-        EPS_CUDA(cudaGetLastError());
-        ++*launches;
-      }
-      planned = true;
-    }
-    const auto kernel = metric == EPS_METRIC_IP ? inverted_score_kernel<EPS_METRIC_IP> : inverted_score_kernel<EPS_METRIC_COSINE>;
-    kernel<<<static_cast<unsigned>(blocks), kInvThreads, 0, ix->stream>>>(ix->d_inv_post, ix->s_inv_plan.as<longlong2>(),
-                                                                         scan.q.ptr, scan.q.elems + elem_base, elem_base,
-                                                                         scan.q.norm2, ix->d_sp_norm2, nq, row_start,
-                                                                         covered, D, ldd);
+int InvertedDist::plan(Index* ix, uint64_t* launches) const {
+  if (planned) return EPS_OK;
+  EPS_TRY(ix->s_inv_plan.reserve(static_cast<size_t>(n_elems) * sizeof(longlong2)));
+  if (n_elems > 0) {
+    inverted_plan_kernel<<<blocks_for(n_elems, 256), 256, 0, ix->stream>>>(
+        ix->d_inv_terms, ix->inv_terms, ix->d_inv_ptr, scan.q.elems + elem_base, n_elems, ix->s_inv_plan.as<longlong2>());
     EPS_CUDA(cudaGetLastError());
     ++*launches;
   }
+  planned = true;
+  return EPS_OK;
+}
+
+namespace {
+
+// Rows of [row_start, row_start + n) the posting lists cover: the first ones.
+int64_t covered_rows(const Index* ix, int64_t row_start, int64_t n) {
+  return std::max<int64_t>(0, std::min(row_start + n, ix->inv_rows) - row_start);
+}
+
+// One CTA per (query, slice of kInvSlice of the n rows), the queries of a slice adjacent.
+int slice_blocks(int64_t nq, int64_t n, unsigned* blocks) {
+  const int64_t b = nq * ((n + kInvSlice - 1) / kInvSlice);
+  if (b > 0x7fffffffll) return fail(EPS_ERR_UNSUPPORTED, "posting lists: too many queries in one launch");
+  *blocks = static_cast<unsigned>(b);
+  return EPS_OK;
+}
+
+// The score kernel over the covered rows [row_start, row_start + covered).
+int score(Index* ix, const InvertedDist& inv, int metric, int64_t row_start, int64_t covered, float* D, int64_t ldd,
+          uint64_t* launches) {
+  unsigned blocks = 0;
+  EPS_TRY(slice_blocks(inv.scan.nq, covered, &blocks));
+  EPS_TRY(inv.plan(ix, launches));
+  const auto kernel = metric == EPS_METRIC_IP       ? inverted_score_kernel<EPS_METRIC_IP>
+                      : metric == EPS_METRIC_COSINE ? inverted_score_kernel<EPS_METRIC_COSINE>
+                                                    : inverted_score_kernel<EPS_METRIC_L2>;
+  const SparseQueries& q = inv.scan.q;
+  kernel<<<blocks, kInvThreads, 0, ix->stream>>>(ix->d_inv_post, ix->s_inv_plan.as<longlong2>(), q.ptr,
+                                                 q.elems + inv.elem_base, inv.elem_base, q.norm2, ix->d_sp_norm2,
+                                                 ix->d_sp_ptr, inv.scan.nq, row_start, covered, D, ldd);
+  EPS_CUDA(cudaGetLastError());
+  ++*launches;
+  return EPS_OK;
+}
+
+// The handle's count of re-scored pairs, created at its first use.
+int rescored_counter(Index* ix, unsigned long long** p) {
+  if (!ix->d_l2_rescored) {
+    EPS_TRY(ix->d_l2_rescored.reserve(8));
+    EPS_CUDA(cudaMemsetAsync(ix->d_l2_rescored, 0, 8, ix->stream));
+  }
+  *p = ix->d_l2_rescored;
+  return EPS_OK;
+}
+
+}  // namespace
+
+int InvertedDist::launch(Index* ix, int metric, int64_t row_start, int64_t n, float* D, int64_t ldd,
+                         uint64_t* launches) const {
+  if (n <= 0 || scan.nq <= 0) return EPS_OK;
+  const int64_t covered = covered_rows(ix, row_start, n);
+  if (covered > 0) {
+    if (metric != EPS_METRIC_IP && metric != EPS_METRIC_COSINE)
+      return fail(EPS_ERR_UNSUPPORTED, "inverted index: only inner-product and cosine distances are read from postings");
+    EPS_TRY(score(ix, *this, metric, row_start, covered, D, ldd, launches));
+  }
   if (covered < n) return scan.launch(ix, metric, row_start + covered, n - covered, D + covered, ldd, launches);
+  return EPS_OK;
+}
+
+int SparseL2Screen::bounds(Index* ix, int64_t row_start, int64_t n, float* D, int64_t ldd, uint64_t* launches) const {
+  if (n <= 0 || inv.scan.nq <= 0) return EPS_OK;
+  const int64_t covered = covered_rows(ix, row_start, n);
+  if (covered > 0) EPS_TRY(score(ix, inv, EPS_METRIC_L2, row_start, covered, D, ldd, launches));
+  if (covered < n)
+    return inv.scan.launch(ix, EPS_METRIC_L2, row_start + covered, n - covered, D + covered, ldd, launches);
+  return EPS_OK;
+}
+
+int SparseL2Screen::threshold(Index* ix, const unsigned long long* keys, int k, float* T, uint64_t* launches) const {
+  const SparseQueries& q = inv.scan.q;
+  if (inv.scan.nq <= 0) return EPS_OK;
+  if (inv.scan.nq > 0x7fffffffll) return fail(EPS_ERR_UNSUPPORTED, "L2 screen: too many queries in one launch");
+  unsigned long long* cnt = nullptr;
+  EPS_TRY(rescored_counter(ix, &cnt));
+  l2_threshold_kernel<<<static_cast<unsigned>(inv.scan.nq), kL2Threads, 0, ix->stream>>>(
+      ix->d_sp_ptr, ix->d_sp_elems, ix->inv_rows, q.ptr, q.elems, keys, k, T, cnt);
+  EPS_CUDA(cudaGetLastError());
+  ++*launches;
+  return EPS_OK;
+}
+
+int SparseL2Screen::rescore(Index* ix, int64_t row_start, int64_t n, float* D, int64_t ldd, const float* T,
+                            const uint32_t* pass, int64_t pass_base, int64_t self_base, uint64_t* launches) const {
+  const int64_t covered = n > 0 ? covered_rows(ix, row_start, n) : 0;
+  if (covered <= 0 || inv.scan.nq <= 0) return EPS_OK;
+  unsigned blocks = 0;
+  EPS_TRY(slice_blocks(inv.scan.nq, covered, &blocks));
+  unsigned long long* cnt = nullptr;
+  EPS_TRY(rescored_counter(ix, &cnt));
+  const SparseQueries& q = inv.scan.q;
+  l2_rescore_kernel<<<blocks, kL2Threads, 0, ix->stream>>>(ix->d_sp_ptr, ix->d_sp_elems, q.ptr, q.elems, T, pass,
+                                                           pass_base, self_base, inv.scan.nq, row_start, covered, D,
+                                                           ldd, cnt);
+  EPS_CUDA(cudaGetLastError());
+  ++*launches;
   return EPS_OK;
 }
 

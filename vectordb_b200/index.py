@@ -245,7 +245,8 @@ class SparseIndex(Index):
     """Device mirror of one sparse-vector field (eps_index_create_sparse): rows are appended as CSR.  Searches are exact
     scans by default; set_search_mode("graph") searches the graph that build() installed where the reference would
     (n_indexed >= 512, no prefilter / force_brute), with the reference's results at IntraQueryThreads = 1.
-    build_inverted() gives an IP or cosine index posting lists that the exact scans read, with the same results.  Config,
+    build_inverted() gives an IP or cosine index posting lists that the exact scans read, and build_l2_screen() gives an
+    L2 index posting lists that screen the exact scans' rows with a proven lower bound, both with the same results.  Config,
     deleted bits, attributes, string codes and dictionary, facets, build and get_graph work as on Index."""
 
     def __init__(self, metric, dim, capacity=0, device=0):
@@ -271,6 +272,19 @@ class SparseIndex(Index):
         r, t, p = C.c_int64(0), C.c_int64(0), C.c_int64(0)
         check(self.L.eps_index_sparse_inverted_info(self.h, C.byref(r), C.byref(t), C.byref(p)))
         return dict(rows=int(r.value), terms=int(t.value), postings=int(p.value))
+
+    def build_l2_screen(self, n=None):
+        """Posting lists of rows [0, n) (None: every mirrored row; 0 drops them) for an L2 index
+        (eps_index_build_sparse_l2_screen).  Results do not change; the exact scans and the build's kNN pass re-score
+        only the covered rows whose proven lower bound can still place them among the k best.  Rows appended later are
+        merged until the next build."""
+        check(self.L.eps_index_build_sparse_l2_screen(self.h, self.rows if n is None else int(n)))
+
+    def l2_screen_info(self):
+        """dict(rows=rows covered (0: no screen), rescored=(query, row) pairs this handle has re-scored so far)."""
+        r, c = C.c_int64(0), C.c_uint64(0)
+        check(self.L.eps_index_sparse_l2_screen_info(self.h, C.byref(r), C.byref(c)))
+        return dict(rows=int(r.value), rescored=int(c.value))
 
     def append(self, rows, first_row=None):
         """Append CSR rows (scipy CSR or (offsets, indices, values)) after the rows already mirrored."""

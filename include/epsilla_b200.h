@@ -82,7 +82,8 @@ typedef struct eps_stats {
   double kernel_ms;    /* device time of the dominant kernel(s) of this call (CUDA events) */
   double total_ms;     /* device time of the whole call incl. copies (CUDA events) */
   uint64_t kernel_launches; /* launches of this call's search, the LIKE match pass included */
-  uint64_t n_redone;   /* exact scan: queries the coarse-pass guard sent back (fp32 scan or a larger candidate list) */
+  uint64_t n_redone;   /* exact scan: queries the coarse-pass guard sent back (fp32 scan or a larger candidate list);
+                          EPS_FILTER_SEARCH_COLLECT: queries answered by the scan over the passing rows */
 } eps_stats;
 
 /* Graph-build parameters.  Defaults (pass NULL) follow NSGConfig(45, 50, 300, 100) and the
@@ -214,6 +215,27 @@ EPS_API int eps_index_config(eps_index* ix, int64_t L_master, int64_t L_local, i
  * every run. */
 EPS_API int eps_index_set_search_width(eps_index* ix, int width);
 
+/* How the graph branch of a filtered dense search answers (eps_search_batch, eps_search_batch_device and, through it,
+ * eps_search_batch_sharded).  It applies only where the reference searches its graph (n_indexed >= 512, no prefilter,
+ * no force_brute) and the filter is non-empty; every other call is unchanged.  A view copies the mode at creation and
+ * may set its own.
+ *   EPS_FILTER_SEARCH_POST (default): the reference's post-filter (vec_search_executor.cpp:906-927).  The page holds the
+ *     passing rows of the unfiltered queue of L candidates, so a selective filter can return fewer than `limit` rows
+ *     even when enough rows pass.
+ *   EPS_FILTER_SEARCH_COLLECT: every query returns min(cap, P) rows, cap = min(n_indexed, limit, L_local, L) and P = the
+ *     rows that are not deleted and pass the filter.  The graph search navigates as in POST and also keeps the best cap
+ *     passing rows among all the rows it evaluates; the passing rows appended after the build are merged in exactly.
+ *     A query left with fewer than min(cap, P) rows, or every query when P is small, is answered by an exact scan of
+ *     the passing rows alone, with the distances of the prefilter scan under eps_index_set_coarse(0);
+ *     eps_stats.n_redone counts those queries.  Results are ascending by (distance, id).  POST's rows of a query are
+ *     the first rows of COLLECT's for the same query when every row is indexed and the query was not scanned.
+ *     A filter whose root compares "@distance" fails with EPS_ERR_UNSUPPORTED before any launch.  The call
+ *     synchronises the index's stream (to read P and the number of short queries), whatever `sync` says.
+ * A sparse index, an unknown mode or a null index: EPS_ERR_INVALID_ARGUMENT. */
+#define EPS_FILTER_SEARCH_POST 0
+#define EPS_FILTER_SEARCH_COLLECT 1
+EPS_API int eps_index_set_filter_search(eps_index* ix, int mode);
+
 /* Launch geometry of the graph-search kernel (performance knob, never changes results): ring_slots = shared-memory row slots per CTA that TMA
  * bulk copies land in (0 = auto: ~48 KB of rows), ctas_per_sm = cap on resident CTAs, i.e. in-flight queries, per SM
  * (0 = whatever fits).  No reference counterpart (the CPU executor has no such geometry). */
@@ -270,7 +292,8 @@ EPS_API int eps_search_batch(eps_index* ix, const float* queries, int64_t nq, in
                      int64_t n_filter, int64_t* out_ids, double* out_dists, int64_t* out_counts, eps_stats* stats);
 
 /* Same search with DEVICE-resident queries and outputs (ids int64, dists float, counts int64),
- * asynchronous on the index's stream unless sync != 0.  For pipelines that keep queries in HBM and
+ * asynchronous on the index's stream unless sync != 0 (a filtered call in EPS_FILTER_SEARCH_COLLECT that takes the
+ * graph branch synchronises the stream in any case).  For pipelines that keep queries in HBM and
  * for the multi-GPU exchange (the per-shard results feed an NCCL all-gather). */
 EPS_API int eps_search_batch_device(eps_index* ix, const float* d_queries, int64_t nq, int64_t limit,
                             const eps_filter_node* filter, int64_t n_filter, int64_t* d_out_ids, float* d_out_dists,
@@ -349,7 +372,7 @@ EPS_API int eps_pair_distances(int device, int metric, const float* a, const flo
  * These calls work on a sparse index as on a dense one: eps_index_set_deleted, eps_index_set_attrs,
  * eps_index_set_string_codes, eps_index_config, eps_index_create_view (the view shares the CSR), eps_index_build,
  * eps_index_get_graph, eps_index_rows, eps_facet_batch.  The dense-only calls (sync_rows, adopt_device_rows,
- * device_rows, set_graph, extend_graph, set_coarse, set_search_width, set_graph_tuning, eps_search_batch*,
+ * device_rows, set_graph, extend_graph, set_coarse, set_search_width, set_filter_search, set_graph_tuning, eps_search_batch*,
  * eps_search_batch_sharded) fail with EPS_ERR_INVALID_ARGUMENT (device_rows returns NULL).
  * --------------------------------------------------------------------------------------------- */
 

@@ -461,10 +461,10 @@ static const SimtKernels kSimt[2][2] = {{{bf_dist_rows_kernel<false, false>, bf_
                                          {bf_dist_rows_kernel<true, true>, bf_dist_tile_kernel<true, true>}}};
 
 int launch_distances(Index* ix, int metric, const float* A_base, int64_t row_start, int64_t n, const float* d_queries,
-                     int64_t nq, float* D, int64_t ldd, uint64_t* launches) {
+                     int64_t nq, float* D, int64_t ldd, uint64_t* launches, int64_t form_nq) {
   const int dim = static_cast<int>(ix->dim);
   const SimtKernels kern = kSimt[metric == EPS_METRIC_L2][ix->vec4];
-  if (nq <= 16) {
+  if ((form_nq > 0 ? form_nq : nq) <= 16) {
     int qt_cap = static_cast<int>(std::min<int64_t>(kRowsQT, (200 * 1024) / (ix->dim * 4)));
     if (qt_cap < 1) return fail(EPS_ERR_UNSUPPORTED, "dimension too large for the brute-force row kernel");
     for (int64_t q0 = 0; q0 < nq; q0 += qt_cap) {
@@ -811,6 +811,162 @@ int exact_topk(Index* ix, const ScanRequest& r, unsigned long long* d_topk, eps_
     return EPS_OK;
   }
   return scan_batch(ix, r, d_topk, stats);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Collect mode of a filtered graph search (capi.cu): the pass bitmap of every row and its popcount P, then the exact
+// top-k over the passing rows alone.  The bitmap is compacted into an ascending id list by two launches (counts per
+// CTA span, then each CTA writes its ids after the counts of the spans before it).
+// ------------------------------------------------------------------------------------------------
+constexpr int kCompactThreads = 256, kCompactWords = 4;
+constexpr int kCompactSpan = kCompactThreads * kCompactWords;  // bitmap words per CTA
+
+__device__ __forceinline__ int span_count(const uint32_t* __restrict__ pass, int64_t words, int64_t w0) {
+  int c = 0;
+#pragma unroll
+  for (int j = 0; j < kCompactWords; ++j)
+    if (w0 + j < words) c += __popc(pass[w0 + j]);
+  return c;
+}
+
+__global__ void __launch_bounds__(kCompactThreads) pass_count_kernel(const uint32_t* __restrict__ pass, int64_t words,
+                                                                     int* __restrict__ counts, unsigned long long* __restrict__ total) {
+  __shared__ int s_sum;
+  if (threadIdx.x == 0) s_sum = 0;
+  __syncthreads();
+  const int c = span_count(pass, words, static_cast<int64_t>(blockIdx.x) * kCompactSpan + threadIdx.x * kCompactWords);
+  if (c) atomicAdd(&s_sum, c);
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    counts[blockIdx.x] = s_sum;
+    if (s_sum) atomicAdd(total, static_cast<unsigned long long>(s_sum));
+  }
+}
+
+__global__ void __launch_bounds__(kCompactThreads) pass_compact_kernel(const uint32_t* __restrict__ pass, int64_t words,
+                                                                       const int* __restrict__ counts, int32_t* __restrict__ ids) {
+  __shared__ int s_base, s_warp[kCompactThreads / 32];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  if (tid == 0) s_base = 0;
+  __syncthreads();
+  int before = 0;
+  for (unsigned b = tid; b < blockIdx.x; b += kCompactThreads) before += counts[b];
+  if (before) atomicAdd(&s_base, before);
+  const int64_t w0 = static_cast<int64_t>(blockIdx.x) * kCompactSpan + tid * kCompactWords;
+  const int c = span_count(pass, words, w0);
+  int x = c;  // inclusive scan of the thread counts: warp, then the warp totals
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const int y = __shfl_up_sync(kFull, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) s_warp[warp] = x;
+  __syncthreads();
+  int o = s_base + x - c;
+  for (int w = 0; w < warp; ++w) o += s_warp[w];
+#pragma unroll
+  for (int j = 0; j < kCompactWords; ++j) {
+    if (w0 + j >= words) break;
+    uint32_t bits = pass[w0 + j];
+    while (bits) {
+      ids[o++] = static_cast<int32_t>((w0 + j) * 32 + __ffs(bits) - 1);
+      bits &= bits - 1;
+    }
+  }
+}
+
+// key (distance, list index) -> (distance, row id): the list is ascending, so the (distance, id) order is unchanged
+__global__ void list_to_row_keys_kernel(unsigned long long* __restrict__ keys, int64_t n, const int32_t* __restrict__ ids) {
+  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (i >= n) return;
+  const unsigned long long k = keys[i];
+  if ((k & kKeyMask) != kKeyInf) keys[i] = (k & 0xffffffff00000000ull) | static_cast<uint32_t>(ids[key_id(k)]);
+}
+
+int collect_pass(Index* ix, const ScanRequest& r, int64_t* P, uint64_t* launches) {
+  const int64_t n = r.row_end, words = (n + 31) / 32, spans = std::max<int64_t>(1, (words + kCompactSpan - 1) / kCompactSpan);
+  EPS_TRY(ix->s_cpass.reserve(static_cast<size_t>(words) * 4));
+  EPS_TRY(ix->s_ccount.reserve(8 + static_cast<size_t>(spans) * 4));
+  unsigned long long* d_total = ix->s_ccount.as<unsigned long long>();
+  EPS_CUDA(cudaMemsetAsync(d_total, 0, 8, ix->stream));
+  if (words > 0) {
+    pass_bitmap_kernel<<<static_cast<unsigned>((words + 127) / 128), 128, 0, ix->stream>>>(
+        ix->any_deleted ? ix->d_deleted.as<const uint8_t>() : nullptr, ix->deleted_bytes, r.d_prog, ix->d_attrs, ix->attr_stride, 0, n,
+        ix->s_cpass.as<uint32_t>());
+    pass_count_kernel<<<static_cast<unsigned>(spans), kCompactThreads, 0, ix->stream>>>(
+        ix->s_cpass.as<uint32_t>(), words, reinterpret_cast<int*>(d_total + 1), d_total);
+    EPS_CUDA(cudaGetLastError());
+    *launches += 2;
+  }
+  unsigned long long h = 0;
+  EPS_CUDA(cudaMemcpyAsync(&h, d_total, 8, cudaMemcpyDeviceToHost, ix->stream));
+  EPS_CUDA(cudaStreamSynchronize(ix->stream));
+  *P = static_cast<int64_t>(h);
+  return EPS_OK;
+}
+
+// The distance tile of list entries [row_start, row_start + n): the listed rows are gathered into ix->s_gather in
+// pieces of at most 64 MB and scanned by the fp32 kernel that a batch of form_nq queries takes.
+struct PassingRowsDist : DistProducer {
+  const int32_t* ids;
+  const float* queries;
+  int64_t nq, form_nq;
+  int launch(Index* ix, int metric, int64_t row_start, int64_t n, float* D, int64_t ldd, uint64_t* launches) const override {
+    const int64_t piece = std::min(n, std::max<int64_t>(kBM, (64ll << 20) / (ix->dim * 4) / kBM * kBM));
+    EPS_TRY(ix->s_gather.reserve(static_cast<size_t>(piece) * ix->dim * 4));
+    for (int64_t s0 = 0; s0 < n; s0 += piece) {
+      const int64_t sn = std::min(piece, n - s0);
+      EPS_TRY(gather_rows(ix, ids + row_start + s0, sn, ix->s_gather.as<float>()));
+      ++*launches;
+      EPS_TRY(launch_distances(ix, metric, ix->s_gather.as<float>(), 0, sn, queries, nq, D + s0, ldd, launches, form_nq));
+    }
+    return EPS_OK;
+  }
+};
+
+int passing_topk(Index* ix, const float* queries, int64_t nq, const int* d_idx, int64_t nb, int64_t k, int64_t P,
+                 unsigned long long* d_topk, eps_stats* stats) {
+  uint64_t launches = 0;
+  const int64_t words = (ix->n_rows + 31) / 32, spans = (words + kCompactSpan - 1) / kCompactSpan;
+  EPS_TRY(ix->s_cids.reserve(static_cast<size_t>(P) * 4));
+  if (P > 0) {
+    pass_compact_kernel<<<static_cast<unsigned>(spans), kCompactThreads, 0, ix->stream>>>(
+        ix->s_cpass.as<uint32_t>(), words, reinterpret_cast<const int*>(ix->s_ccount.as<unsigned long long>() + 1), ix->s_cids.as<int32_t>());
+    EPS_CUDA(cudaGetLastError());
+    ++launches;
+  }
+  DevBuf d_q, d_res;
+  const float* q = queries;
+  unsigned long long* res = d_topk;
+  if (d_idx) {  // the picked queries, and their lists scattered back below
+    EPS_TRY(d_q.reserve(static_cast<size_t>(nb) * ix->dim * 4));
+    EPS_TRY(d_res.reserve(static_cast<size_t>(nb) * k * 8));
+    const int64_t tot = nb * ix->dim;
+    gather_queries_kernel<<<static_cast<unsigned>((tot + 255) / 256), 256, 0, ix->stream>>>(queries, d_idx, static_cast<int>(nb),
+                                                                                          static_cast<int>(ix->dim), d_q.as<float>());
+    EPS_CUDA(cudaGetLastError());
+    ++launches;
+    q = d_q.as<float>();
+    res = d_res.as<unsigned long long>();
+  }
+  PassingRowsDist dist;
+  dist.ids = ix->s_cids.as<int32_t>(); dist.queries = q; dist.nq = nb; dist.form_nq = nq;
+  ScanRequest s;
+  s.dist = &dist; s.nq = nb; s.row_start = 0; s.row_end = P; s.k = k; s.metric = ix->metric; s.skip_deleted = false;
+  EPS_TRY(fp32_scan(ix, s, res, stats));
+  const int64_t tk = nb * k;
+  list_to_row_keys_kernel<<<static_cast<unsigned>((tk + 255) / 256), 256, 0, ix->stream>>>(res, tk, ix->s_cids.as<int32_t>());
+  EPS_CUDA(cudaGetLastError());
+  ++launches;
+  if (d_idx) {
+    scatter_keys_kernel<<<static_cast<unsigned>((tk + 255) / 256), 256, 0, ix->stream>>>(res, d_idx, static_cast<int>(nb),
+                                                                                       static_cast<int>(k), d_topk);
+    EPS_CUDA(cudaGetLastError());
+    ++launches;
+    EPS_CUDA(cudaStreamSynchronize(ix->stream));  // the temporaries die with this frame
+  }
+  if (stats) stats->kernel_launches += launches;
+  return EPS_OK;
 }
 
 }  // namespace eps

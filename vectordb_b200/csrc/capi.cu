@@ -2,6 +2,7 @@
 // VecSearchExecutor::Search orchestration (engine/db/execution/vec_search_executor.cpp:833-935).
 #include <cmath>
 #include <cstdio>
+#include <cstdlib>
 #include <algorithm>
 #include <cstring>
 #include <memory>
@@ -258,6 +259,61 @@ struct SparseBatch : QueryBatch {
   }
 };
 
+// Below this many passing rows, a collect-mode call answers the whole batch by the scan over the passing rows, which
+// costs nq x P distances; above it the graph search runs and only the queries it leaves short are scanned (DESIGN.md
+// §K3).  EPS_COLLECT_SCAN_ROWS overrides it (developer knob: tools/filtered_check.py times both sides with it).
+constexpr int64_t kCollectScanRows = 65536;
+static int64_t collect_scan_rows() {
+  const char* e = getenv("EPS_COLLECT_SCAN_ROWS");
+  return e ? atoll(e) : kCollectScanRows;
+}
+
+// EPS_FILTER_SEARCH_COLLECT: the graph branch of a filtered dense search that returns min(cap, P) rows per query, P = the
+// rows that are not deleted and pass the filter.  The keys go to ix->s_ckeys [nq x cap] for finalize_keys.
+//   1. the pass bitmap of rows [0, total) and P;
+//   2. P <= collect_scan_rows(): the exact scan over the passing rows answers every query;
+//   3. otherwise the graph search keeps, per query, the best cap passing rows it evaluates, and
+//   4. the filtered tail scan of rows [n_indexed, total) is merged in exactly;
+//   5. queries left with fewer than min(cap, P) rows are answered by the scan over the passing rows.
+// eps_stats.n_redone counts the queries answered in 2 or 5.
+static int collect_search(Index* ix, ScanRequest scan, int64_t L, int64_t cap, eps_stats* local, eps_stats* stats) {
+  if (cap > 8192) return fail(EPS_ERR_UNSUPPORTED, "collect filter search: more than 8192 results per query are not supported");
+  const int64_t nq = scan.nq, total = ix->n_rows, n_indexed = ix->n_indexed;
+  scan.row_start = 0; scan.row_end = total;
+  int64_t P = 0;
+  EPS_TRY(collect_pass(ix, scan, &P, &local->kernel_launches));
+  EPS_TRY(ix->s_ckeys.reserve(static_cast<size_t>(nq) * cap * 8));
+  unsigned long long* keys = ix->s_ckeys.as<unsigned long long>();
+  if (P <= collect_scan_rows()) {
+    EPS_TRY(passing_topk(ix, scan.queries, nq, nullptr, nq, cap, P, keys, local));
+    local->n_redone += static_cast<uint64_t>(nq);
+    if (stats) EPS_CUDA(cudaEventRecord(ix->ev[2], ix->stream));
+    return EPS_OK;
+  }
+  EPS_TRY(ix->s_queue.reserve(static_cast<size_t>(nq) * L * 8));
+  EPS_TRY(ix->s_clist.reserve(static_cast<size_t>(nq) * cap * 8));
+  const GraphCollect gc{ix->s_cpass.as<uint32_t>(), ix->s_clist.as<unsigned long long>(), cap};
+  EPS_TRY(graph_search(ix, scan.queries, nq, L, ix->s_queue.as<unsigned long long>(), local, &gc));
+  ix->graph_counters_pending = true;
+  if (stats) EPS_CUDA(cudaEventRecord(ix->ev[2], ix->stream));
+  int64_t tail_k = 0;
+  if (total > n_indexed) {
+    tail_k = std::min<int64_t>(cap, total - n_indexed);
+    EPS_TRY(ix->s_tail.reserve(static_cast<size_t>(nq) * tail_k * 8));
+    scan.row_start = n_indexed; scan.k = tail_k;
+    EPS_TRY(exact_topk(ix, scan, ix->s_tail.as<unsigned long long>(), local));
+  }
+  const int* d_short = nullptr;
+  int64_t n_short = 0;
+  EPS_TRY(collect_merge(ix, gc.out, ix->s_tail.as<unsigned long long>(), nq, cap, tail_k, P, keys, &d_short, &n_short));
+  local->kernel_launches += 1;
+  if (n_short > 0) {
+    EPS_TRY(passing_topk(ix, scan.queries, nq, d_short, n_short, cap, P, keys, local));
+    local->n_redone += static_cast<uint64_t>(n_short);
+  }
+  return EPS_OK;
+}
+
 // VecSearchExecutor::Search (:833-935) of nq queries into device ids / dists / counts.  ev[1] -> ev[2] brackets the
 // search kernels when stats are wanted.
 static int run_search(Index* ix, const QueryBatch& qb, int64_t nq, int64_t limit, const eps_filter_node* filter,
@@ -266,6 +322,15 @@ static int run_search(Index* ix, const QueryBatch& qb, int64_t nq, int64_t limit
   if (limit < 1) return fail(EPS_ERR_INVALID_ARGUMENT, "limit must be >= 1");
   FilterProg h_prog;
   EPS_TRY(lower_filter(filter, n_filter, &h_prog));
+  const int64_t total = ix->n_rows;
+  const int64_t n_indexed = ix->n_indexed;
+  // BruteforceThreshold (hpp:28); a sparse index in EPS_SPARSE_SEARCH_SCAN always scans, whatever graph is installed
+  const bool graph = !ix->prefilter && !ix->force_brute && n_indexed >= 512 &&
+                     (!ix->sparse || ix->sparse_search == EPS_SPARSE_SEARCH_GRAPH);
+  const bool collect = graph && !ix->sparse && h_prog.n > 0 && ix->filter_search == EPS_FILTER_SEARCH_COLLECT;
+  if (collect && h_prog.root_uses_dist)
+    return fail(EPS_ERR_UNSUPPORTED, "collect filter search: a filter whose root compares @distance cannot be decided before "
+                                     "the distance is known (use EPS_FILTER_SEARCH_POST)");
   const FilterProg* d_prog = nullptr;
   uint64_t like_launches = 0;
   if (h_prog.n > 0) {
@@ -277,18 +342,18 @@ static int run_search(Index* ix, const QueryBatch& qb, int64_t nq, int64_t limit
     // from pageable memory is staged synchronously by the runtime, so it is safe.
     d_prog = ix->s_filter.as<FilterProg>();
   }
-  const int64_t total = ix->n_rows;
-  const int64_t n_indexed = ix->n_indexed;
   eps_stats local;
   std::memset(&local, 0, sizeof(local));
   local.kernel_launches = like_launches;  // the LIKE pass
   ScanRequest scan = qb.scan;
   scan.metric = ix->metric; scan.d_prog = d_prog; scan.h_prog = &h_prog;
   if (stats) EPS_CUDA(cudaEventRecord(ix->ev[1], ix->stream));
-  // BruteforceThreshold (hpp:28); a sparse index in EPS_SPARSE_SEARCH_SCAN always scans, whatever graph is installed
-  const bool graph = !ix->prefilter && !ix->force_brute && n_indexed >= 512 &&
-                     (!ix->sparse || ix->sparse_search == EPS_SPARSE_SEARCH_GRAPH);
-  if (graph) {
+  if (collect) {
+    const int64_t L = std::min<int64_t>(ix->L_master, n_indexed);
+    const int64_t cap = std::min<int64_t>(std::min<int64_t>(std::min<int64_t>(n_indexed, limit), ix->L_local), L);
+    EPS_TRY(collect_search(ix, scan, L, cap, &local, stats));
+    EPS_TRY(finalize_keys(ix, ix->s_ckeys.as<unsigned long long>(), nq, cap, limit, cap, d_ids, d_dists, d_counts));
+  } else if (graph) {
     // :869-933: graph search, exact scan of the rows appended after the build, merge of the two and post-filter walk
     const int64_t L = std::min<int64_t>(ix->L_master, n_indexed);  // Q1 clamp
     // :872 min(n_indexed, limit, L_local); the queue row holds L entries, so the merge window is clamped to it
@@ -926,6 +991,16 @@ int eps_index_set_search_width(eps_index* h, int width) {
   EPS_TRY(eps::dense_only(ix));
   if (width < 1 || width > 8) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "search width must be in [1, 8]");
   ix->search_width = width;
+  return EPS_OK;
+}
+
+int eps_index_set_filter_search(eps_index* h, int mode) {
+  Index* ix = reinterpret_cast<Index*>(h);
+  if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");
+  if (ix->sparse) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "filter search mode on a sparse index (its default search is exact)");
+  if (mode != EPS_FILTER_SEARCH_POST && mode != EPS_FILTER_SEARCH_COLLECT)
+    return eps::fail(EPS_ERR_INVALID_ARGUMENT, "filter search mode must be 0 (post) or 1 (collect)");
+  ix->filter_search = mode;
   return EPS_OK;
 }
 

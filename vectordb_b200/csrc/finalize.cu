@@ -107,6 +107,30 @@ __global__ void finalize_keys_kernel(const unsigned long long* __restrict__ topk
   if (threadIdx.x == 0) out_counts[q] = cnt;
 }
 
+// Collect mode (capi.cu): one thread per query merges the graph search's list of passing rows with the tail scan's top
+// keys.  Both are ascending and kKeyInf padded, and their rows are disjoint (graph rows < n_indexed <= tail rows), so
+// the first cap keys of the merge are the best cap of the union: no slot quirk of the post-filter merge applies.  A
+// query left with fewer than min(cap, P) keys is listed in short_idx.
+__global__ void collect_merge_kernel(const unsigned long long* __restrict__ list, const unsigned long long* __restrict__ tail,
+                                     int nq, int cap, int tail_k, int64_t P, unsigned long long* __restrict__ out,
+                                     int* __restrict__ short_idx, int* __restrict__ n_short) {
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= nq) return;
+  const unsigned long long* a = list + static_cast<int64_t>(q) * cap;
+  const unsigned long long* b = tail ? tail + static_cast<int64_t>(q) * tail_k : nullptr;
+  unsigned long long* o = out + static_cast<int64_t>(q) * cap;
+  int i = 0, j = 0, n = 0;
+  for (int t = 0; t < cap; ++t) {
+    const unsigned long long x = i < cap ? a[i] & kKeyMask : kKeyInf;
+    const unsigned long long y = j < tail_k ? b[j] & kKeyMask : kKeyInf;
+    unsigned long long z;
+    if (x <= y) { z = x; ++i; } else { z = y; ++j; }
+    o[t] = z;
+    n += z != kKeyInf;
+  }
+  if (n < min(static_cast<int64_t>(cap), P)) short_idx[atomicAdd(n_short, 1)] = q;
+}
+
 // k-way merge of n_shards sorted lists per query (ids are GLOBAL int64).  One CTA per query, bitonic
 // sort of the (ordered-distance, id) pairs in shared memory.
 __global__ void merge_shards_kernel(const int64_t* __restrict__ ids, const float* __restrict__ dists, int n_shards,
@@ -177,6 +201,23 @@ int finalize_keys(Index* ix, const unsigned long long* d_topk, int64_t nq, int64
                                                                         static_cast<int>(limit), static_cast<int>(cap),
                                                                         d_ids, d_dists, d_counts);
   EPS_CUDA(cudaGetLastError());
+  return EPS_OK;
+}
+
+int collect_merge(Index* ix, const unsigned long long* d_list, const unsigned long long* d_tail, int64_t nq, int64_t cap,
+                  int64_t tail_k, int64_t P, unsigned long long* d_out, const int** d_short_idx, int64_t* n_short) {
+  EPS_TRY(ix->s_cshort.reserve(static_cast<size_t>(nq + 1) * 4));  // [count | query indices]
+  int* d_n = ix->s_cshort.as<int>();
+  *d_short_idx = d_n + 1;
+  EPS_CUDA(cudaMemsetAsync(d_n, 0, 4, ix->stream));
+  collect_merge_kernel<<<static_cast<unsigned>((nq + 127) / 128), 128, 0, ix->stream>>>(
+      d_list, tail_k > 0 ? d_tail : nullptr, static_cast<int>(nq), static_cast<int>(cap), static_cast<int>(tail_k), P, d_out,
+      d_n + 1, d_n);
+  EPS_CUDA(cudaGetLastError());
+  int h = 0;
+  EPS_CUDA(cudaMemcpyAsync(&h, d_n, 4, cudaMemcpyDeviceToHost, ix->stream));
+  EPS_CUDA(cudaStreamSynchronize(ix->stream));
+  *n_short = h;
   return EPS_OK;
 }
 

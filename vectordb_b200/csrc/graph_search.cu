@@ -108,7 +108,13 @@ struct GSArgs {
   int64_t n_sk;                   // rows sketched (n_indexed)
   float sk_g, sk_scale;           // rounded-down factors of the bound (see screen_fresh)
   unsigned long long* n_screened; // ids the screen dropped, summed over every search of the handle
+  // collect mode (kCollect): besides the queue, each query keeps the best `cap` keys of the passing rows it evaluates
+  const uint32_t* pass;           // bit i: row i is not deleted and passes the filter
+  unsigned long long* out_r;      // [nq x cap] those keys, ascending, kKeyInf padded
+  int cap;
 };
+
+__device__ __forceinline__ bool row_passes(const uint32_t* pass, uint32_t id) { return (pass[id >> 5] >> (id & 31)) & 1u; }
 
 template <bool L2>
 __device__ __forceinline__ void acc4(const float4& x, const float4& y, float& a) {
@@ -166,10 +172,12 @@ __device__ __forceinline__ void warp_rows_scalar(const float* const (&rows)[S], 
 // |s_x - p_q| - ex_x - E_q <= |P~(x - q)| <= sqrt(1 + eps) |x - q|, and the kernel's fp32 L2 sum of the row is at least
 // (1 - 2 (d + 2) 2^-24) |x - q|^2, so LB never exceeds the distance the consumer would compute.  An id is dropped iff
 // make_key(LB, id) >= bound; the consumer's bound is at most this one, so it would have dropped the id too.  Bit i of
-// keep is set for every id i that stays.
+// keep is set for every id i that stays.  In collect mode the id must also stay out of the passing rows' list: it is
+// dropped only when it fails the filter or make_key(LB, id) >= rbound, the list's worst key (kKeyInf until it is full).
 constexpr int kScreenIds = 64;  // ids whose loads are in flight together (4 per 8-lane group)
+template <bool kCollect>
 __device__ __forceinline__ void screen_fresh(const GSArgs& a, const int* fifo, unsigned fmask, uint32_t tail, int total, const float* psk,
-                                             unsigned long long bound, int tid, unsigned* keep) {
+                                             unsigned long long bound, unsigned long long rbound, int tid, unsigned* keep) {
   const int g = tid >> 3, j = tid & 7;
   constexpr int kPer = kScreenIds / (kGsThreads / 8);
   const float4* sk4 = reinterpret_cast<const float4*>(a.sk);
@@ -207,6 +215,8 @@ __device__ __forceinline__ void screen_fresh(const GSArgs& a, const int* fifo, u
         if (r > 0.f) {  // false for NaN as well
           const float lb = __fmul_rd(__fmul_rd(r, r), a.sk_scale);
           drop = lb <= FLT_MAX && make_key(lb, static_cast<uint32_t>(id[b])) >= bound;
+          if (kCollect && drop)
+            drop = !row_passes(a.pass, static_cast<uint32_t>(id[b])) || make_key(lb, static_cast<uint32_t>(id[b])) >= rbound;
         }
         if (!drop) atomicOr(keep + (i >> 5), 1u << (i & 31));
       }
@@ -215,11 +225,13 @@ __device__ __forceinline__ void screen_fresh(const GSArgs& a, const int* fifo, u
 }
 
 // Consumer step of one warp over its S slots (slot of local index s = cw + 3 s): wait for the landed rows, distances,
-// accepted keys to the pending buffer.  Returns nothing; the caller refills the slots.
-template <int S>
+// accepted keys to the pending buffer; in collect mode, the keys of passing rows under rbound to the list's pending buffer
+// rpend.  Returns nothing; the caller refills the slots.
+template <int S, bool kCollect>
 __device__ __forceinline__ void consume_slots(const GSArgs& a, unsigned occ_mask, unsigned par_mask, int cw, int lane, bool staged,
                                               const unsigned char* ring, uint32_t bar0, const float* qv, const int* slot_id,
-                                              unsigned long long bound, unsigned long long* pend, int* s_npend) {
+                                              unsigned long long bound, unsigned long long* pend, int* s_npend,
+                                              unsigned long long rbound, unsigned long long* rpend, int* s_nrpend) {
   float d[S];
   if (staged) {
 #pragma unroll
@@ -243,14 +255,17 @@ __device__ __forceinline__ void consume_slots(const GSArgs& a, unsigned occ_mask
   if (lane < S && ((occ_mask >> lane) & 1u)) {
     const unsigned long long key = make_key(finish_metric(a.metric, mine), static_cast<uint32_t>(slot_id[cw + 3 * lane]));
     if (key < bound) pend[atomicAdd(s_npend, 1)] = key;  // dist > bound rejected (:424); ties by id
+    if (kCollect && key < rbound && row_passes(a.pass, key_id(key))) rpend[atomicAdd(s_nrpend, 1)] = key;
   }
 }
 
 // Two register budgets of the same kernel: 72 registers per thread allow 7 resident CTAs per SM but spill 376 B per
 // thread to local memory (348 B of spill loads); 128 registers allow 4 and spill 12 B (16 B of loads).  graph_search
 // picks the instance from the geometry it launches.  kScreen: the screen is compiled in only where it runs, so that a
-// search without it (other metrics, tables it cannot pay on) keeps the registers of the kernel without it.
-template <int kMinCtas, bool kScreen>
+// search without it (other metrics, tables it cannot pay on) keeps the registers of the kernel without it.  kCollect: the
+// collect mode of a filtered search (DESIGN.md §K2), which navigates as the other instances do and also keeps each
+// query's list of the best a.cap keys of the passing rows it evaluates, merged like the queue.
+template <int kMinCtas, bool kScreen, bool kCollect = false>
 __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSArgs a) {
   extern __shared__ __align__(128) unsigned char gs_smem[];
   const int dim4p = (a.dim + 3) & ~3;
@@ -265,6 +280,10 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
   int* fifo = pos + kPC;                                                                           // [fc]
   int* slot_id = fifo + a.fc;                                                                      // [kMaxR] row id in each ring slot
   unsigned* ubits = reinterpret_cast<unsigned*>(slot_id + kMaxR);                                  // [(Lp + 31) / 32] unchecked-entry bitmap
+  // collect: [cap] the passing rows' list, [kPC] its pending keys (8-byte aligned after an even number of bitmap words)
+  unsigned long long* rq = reinterpret_cast<unsigned long long*>(ubits + (((a.Lp + 31) / 32 + 1) & ~1));
+  unsigned long long* rpend = rq + a.cap;
+  __shared__ int s_nrpend;
   __shared__ int s_q, s_ncur, s_cursor, s_npend, s_ncont;
   __shared__ unsigned s_head;                      // FIFO entries [s_head, fifo_tail) are not yet issued to the ring
   __shared__ int s_cid[kMaxW];
@@ -342,6 +361,22 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
     block_bitonic_sort(qa, a.Lp);
     for (int w = tid; w < ((L + 31) >> 5); w += kGsThreads)  // every seed starts unchecked
       ubits[w] = (w * 32 + 32 <= L) ? 0xffffffffu : ((1u << (L & 31)) - 1u);
+    if (kCollect) {  // the list starts with the first cap passing seeds of the sorted queue
+      if (warp == 0) {
+        int n = 0;
+        for (int base = 0; base < L && n < a.cap; base += 32) {
+          const int i = base + lane;
+          const unsigned long long key = i < L ? qa[i] : kKeyInf;
+          const bool ok = i < L && row_passes(a.pass, key_id(key));
+          const unsigned b = __ballot_sync(kFull, ok);
+          const int o = n + __popc(b & lane_lt);
+          if (ok && o < a.cap) rq[o] = key;
+          n += __popc(b);
+        }
+        for (int i = min(n, a.cap) + lane; i < a.cap; i += 32) rq[i] = kKeyInf;
+      }
+      if (tid == 0) s_nrpend = 0;
+    }
     if (tid == 0) st_ndist += static_cast<unsigned long long>(L);
     uint32_t fifo_tail = 0;   // ids appended to the FIFO
     uint32_t fresh_n = 0;  // fresh ids of the query (= fifo_tail unless the screen dropped some); the log holds them
@@ -359,6 +394,7 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
       GS_T(tx1);
       GS_ACC(0, tx0, tx1);
       const int m = s_npend;
+      const int rm = kCollect ? s_nrpend : 0;
       const uint32_t head = s_head;
       const int ncont = s_ncont;
       // -- D: merge the pending keys --
@@ -367,6 +403,7 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
       // the snapshot above (the merge's own barriers do that when there is a merge)
       if (merged) merge_pending(qa, pend, cs, pos, m, L, &s_npend, &s_cursor, ubits);
       else __syncthreads();
+      if (kCollect && rm > 0) merge_pending<false>(rq, rpend, cs, pos, rm, a.cap, &s_nrpend, nullptr, nullptr);
       GS_T(tm1);
       GS_ACC(1, tx1, tm1);
       const bool idle = inflight == 0 && head == fifo_tail;
@@ -381,13 +418,17 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
       // buffer (the bound never grows); the merge evicts them, so the queue after the merge is the same.
       if (n_own > 0) {
         const unsigned long long bound = qa[L - 1] & kKeyMask;  // worst entry as of the last merge (:546)
+        const unsigned long long rbound = kCollect ? rq[a.cap - 1] : kKeyInf;
         for (;;) {
           if (occ_mask) {
             GS_T(tw0);
-            if (n_own <= 1) consume_slots<1>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend);
-            else if (n_own <= 2) consume_slots<2>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend);
-            else if (n_own <= 4) consume_slots<4>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend);
-            else consume_slots<8>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend);
+#define GS_CONSUME(S) consume_slots<S, kCollect>(a, occ_mask, par_mask, cw, lane, staged, ring, bar0, qv, slot_id, bound, pend, &s_npend, \
+                                                 rbound, rpend, &s_nrpend)
+            if (n_own <= 1) GS_CONSUME(1);
+            else if (n_own <= 2) GS_CONSUME(2);
+            else if (n_own <= 4) GS_CONSUME(4);
+            else GS_CONSUME(8);
+#undef GS_CONSUME
             par_mask ^= occ_mask;
             GS_T(tw1);
             GS_ACC(3, tw0, tw1);
@@ -418,6 +459,7 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
           const unsigned head_now = *reinterpret_cast<volatile unsigned*>(&s_head);
           const int npend_now = *reinterpret_cast<volatile int*>(&s_npend);
           if (head_now >= fifo_tail || npend_now + R > kPC) break;
+          if (kCollect && *reinterpret_cast<volatile int*>(&s_nrpend) + R > kPC) break;
         }
       }
       if (!want) continue;
@@ -617,7 +659,7 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
       const unsigned long long sbound = kScreen ? qa[L - 1] & kKeyMask : kKeyInf;
       if (kScreen && total > 0 && sbound != kKeyInf) {
         __syncthreads();  // (3) the fresh ids are in the FIFO, s_keep is clear
-        screen_fresh(a, fifo, fmask, fifo_tail, total, psk, sbound, tid, s_keep);
+        screen_fresh<kCollect>(a, fifo, fmask, fifo_tail, total, psk, sbound, kCollect ? rq[a.cap - 1] : kKeyInf, tid, s_keep);
         int mine[kMaxW * kEll / kGsThreads];
 #pragma unroll
         for (int r = 0; r < kMaxW * kEll / kGsThreads; ++r) {
@@ -672,9 +714,13 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
     {
       const int m = s_npend;  // only checked entries can be left (the last pick found nothing unchecked)
       if (m > 0) merge_pending(qa, pend, cs, pos, m, L, &s_npend, &s_cursor, ubits);
+      const int rm = kCollect ? s_nrpend : 0;
+      if (rm > 0) merge_pending<false>(rq, rpend, cs, pos, rm, a.cap, &s_nrpend, nullptr, nullptr);
     }
     unsigned long long* out = a.out_queue + static_cast<int64_t>(q) * L;
     for (int i = tid; i < L; i += kGsThreads) out[i] = qa[i];
+    if (kCollect)
+      for (int i = tid; i < a.cap; i += kGsThreads) a.out_r[static_cast<int64_t>(q) * a.cap + i] = rq[i];
 #ifdef EPS_GS_PROFILE
     if (tid == 0) {
       unsigned long long t;
@@ -805,7 +851,7 @@ int ensure_ell(Index* ix, uint64_t* launches) {
 }
 
 int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsigned long long* d_queue,
-                 eps_stats* stats) {
+                 eps_stats* stats, const GraphCollect* collect) {
   int Lp = 0;
   EPS_TRY(graph_launch_prologue(ix, L, "graph_search", &Lp));
   const int dim = static_cast<int>(ix->dim);
@@ -817,16 +863,27 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   // FIFO: a backlog below R entries + the ids one A step appends (W adjacency rows or one 128-id continuation chunk)
   const int fc = next_pow2(std::max(width * kEll, kGsThreads) + kMaxR);
   const bool screen = screen_on(ix);  // the query sketch takes shared memory only when the screen runs
+  // collect: the passing rows' list and its pending keys after the bitmap words (padded to an even count)
+  const size_t collect_bytes = collect ? 4 + static_cast<size_t>(collect->cap + kPC) * 8 : 0;
   auto smem_for = [&](int r) {
     return static_cast<size_t>(r) * slot_bytes + static_cast<size_t>(Lp) * 8 + 2 * kPC * 8 + kMaxR * 8 +
-           static_cast<size_t>(dimp) * 4 + (screen ? (kSketch + 4) * 4 : 0) + kPC * 4 + static_cast<size_t>(fc) * 4 + kMaxR * 4 + static_cast<size_t>((Lp + 31) / 32) * 4;
+           static_cast<size_t>(dimp) * 4 + (screen ? (kSketch + 4) * 4 : 0) + kPC * 4 + static_cast<size_t>(fc) * 4 + kMaxR * 4 + static_cast<size_t>((Lp + 31) / 32) * 4 +
+           collect_bytes;
   };
   while (R > 2 && smem_for(R) > 200 * 1024) --R;
   if (smem_for(R) > 226 * 1024) return fail(EPS_ERR_UNSUPPORTED, "queue + query + row ring do not fit in shared memory");
-  for (auto k : {graph_search_kernel<7, false>, graph_search_kernel<4, false>, graph_search_kernel<7, true>, graph_search_kernel<4, true>})
-    EPS_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_for(R))));
+  using Kernel = void (*)(GSArgs);
+  // [collect][per_sm <= 4][screen]
+  const Kernel kernels[2][2][2] = {{{graph_search_kernel<7, false>, graph_search_kernel<7, true>},
+                                    {graph_search_kernel<4, false>, graph_search_kernel<4, true>}},
+                                   {{graph_search_kernel<7, false, true>, graph_search_kernel<7, true, true>},
+                                    {graph_search_kernel<4, false, true>, graph_search_kernel<4, true, true>}}};
+  const int ci = collect ? 1 : 0;
+  for (int p = 0; p < 2; ++p)
+    for (int s = 0; s < 2; ++s)
+      EPS_CUDA(cudaFuncSetAttribute(kernels[ci][p][s], cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_for(R))));
   auto resident = [&](int r, int* out) {
-    EPS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(out, graph_search_kernel<7, false>, kGsThreads, smem_for(r)));
+    EPS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(out, kernels[ci][0][0], kGsThreads, smem_for(r)));
     if (*out < 1) *out = 1;
     if (ix->graph_ctas_per_sm > 0) *out = std::min(*out, ix->graph_ctas_per_sm);
     return EPS_OK;
@@ -884,6 +941,9 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   a.W = width; a.R = R; a.slot_bytes = slot_bytes; a.fc = fc;
   a.qtimes = nullptr;
   a.sk = nullptr; a.qsk = nullptr; a.n_sk = 0; a.sk_g = 0.f; a.sk_scale = 0.f; a.n_screened = nullptr;
+  a.pass = collect ? collect->pass : nullptr;
+  a.out_r = collect ? collect->out : nullptr;
+  a.cap = collect ? static_cast<int>(collect->cap) : 0;
   if (screen) {
     if (!ix->d_screened) {
       EPS_TRY(ix->d_screened.reserve(8));
@@ -905,10 +965,7 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   // at most 4 resident CTAs per SM (what the auto rule picks for batches above one wave at 7 per SM, e.g. 1024 queries
   // at L = 768): the register file has room for 128 registers per thread, so the instance that hardly spills runs;
   // smaller batches keep 7 resident queries per SM
-  if (per_sm <= 4 && screen) graph_search_kernel<4, true><<<slots, kGsThreads, smem, ix->stream>>>(a);
-  else if (per_sm <= 4) graph_search_kernel<4, false><<<slots, kGsThreads, smem, ix->stream>>>(a);
-  else if (screen) graph_search_kernel<7, true><<<slots, kGsThreads, smem, ix->stream>>>(a);
-  else graph_search_kernel<7, false><<<slots, kGsThreads, smem, ix->stream>>>(a);
+  kernels[ci][per_sm <= 4 ? 1 : 0][screen ? 1 : 0]<<<slots, kGsThreads, smem, ix->stream>>>(a);
   EPS_CUDA(cudaGetLastError());
   if (stats) {
     stats->n_seed += static_cast<uint64_t>(nq) * static_cast<uint64_t>(L);

@@ -54,7 +54,9 @@ __device__ __forceinline__ bool vset_claim(uint32_t* t, uint32_t mask, uint32_t 
 // Block-wide merge of the m (<= kPC) pending keys into the sorted queue qa[0..L): sort by counting, binary-search
 // the insertion points, shift the tail in place in super-tiles of 8 keys per thread (each key moves right by the
 // number of pending keys that precede it), drop the keys into the holes.  Entries pushed past L are evicted
-// (AddIntoQueue's drop-worst, :104-108).  Returns the lowest insert position through *s_cursor (min).
+// (AddIntoQueue's drop-worst, :104-108).  Returns the lowest insert position through *s_cursor (min).  kQueue = false:
+// a plain sorted list of L keys (the collect mode's passing rows), with no cursor and no unchecked-entry bitmap.
+template <bool kQueue = true>
 __device__ __forceinline__ void merge_pending(unsigned long long* qa, unsigned long long* pend, unsigned long long* cs, int* pos,
                                               int m, int L, int* s_npend, int* s_cursor, unsigned* ubits) {
   const int tid = threadIdx.x;
@@ -94,11 +96,11 @@ __device__ __forceinline__ void merge_pending(unsigned long long* qa, unsigned l
   }
   if (tid == 0) {
     *s_npend = 0;
-    if (p0 < *s_cursor) *s_cursor = p0;
+    if (kQueue && p0 < *s_cursor) *s_cursor = p0;
   }
   __syncthreads();
   // the unchecked-entry bitmap (one bit per queue slot, what the pick scans) from the first changed word on
-  if (p0 < L) {
+  if (kQueue && p0 < L) {
     const int nwords = (L + 31) >> 5, lane = tid & 31;
     for (int w = (p0 >> 5) + (tid >> 5); w < nwords; w += kGsThreads / 32) {
       const int idx = w * 32 + lane;

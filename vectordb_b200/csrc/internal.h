@@ -138,6 +138,7 @@ struct Config {
   int coarse_guard = 1;          // verify the coarse pass after the re-score and redo unsafe queries (brute_force.cu)
   int coarse_boost = 1;          // multiplier of k' learnt by the guard for this table (1, 4, 16, 64)
   int graph_screen = EPS_GRAPH_SCREEN_AUTO;
+  int filter_search = EPS_FILTER_SEARCH_POST;  // graph branch of a filtered dense search: post-filter or collect
 };
 
 // Deleted with its device current (eps_index_destroy): it frees what it owns, never its base's Table.
@@ -170,6 +171,9 @@ struct Index : Table, Config {
   DevBuf s_queries, s_dist, s_topk, s_topk2, s_pass, s_filter, s_vset, s_visited, s_vlog, s_queue, s_tail, s_out_ids, s_out_dists,
       s_out_counts, s_stats, s_misc, s_seed_rows, s_seed_dist, s_xnorm, s_qnorm, s_coarse, s_thr, s_cand, s_cand_cnt, s_bf16, s_qbf16, s_flags,
       s_sparse_q, s_xnorm_max, s_like, s_like_jobs, s_inv_plan, s_l2_screen;
+  // collect mode: the pass bitmap of [0, n_rows), its per-CTA counts and P, the passing ids, the lists of the passing
+  // rows, the merged keys per query, the short queries, and the gathered rows of the scan over passing rows
+  DevBuf s_cpass, s_ccount, s_cids, s_clist, s_ckeys, s_cshort, s_gather;
   int64_t bf16_rows = 0;         // rows converted into s_bf16 while it had generation bf16_gen
   uint64_t bf16_gen = 0;
   int64_t xnorm_rows = 0;        // rows whose |x|^2 is current in s_xnorm; s_xnorm_max holds the largest (float bits)
@@ -218,8 +222,21 @@ int exact_topk(Index* ix, const ScanRequest& r, unsigned long long* d_topk, eps_
 
 // Distances of rows [row_start,row_start+n) of A_base to nq device queries: D[q*ldd + i] (row kernel for
 // nq <= 16, 128x128 tile kernel otherwise).
+// form_nq > 0 picks the kernel as for a batch of form_nq queries: the two kernels add a row's terms in different orders,
+// so a subset of a batch takes the batch's kernel to get the batch's bits.
 int launch_distances(Index* ix, int metric, const float* A_base, int64_t row_start, int64_t n, const float* d_queries,
-                     int64_t nq, float* D, int64_t ldd, uint64_t* launches);
+                     int64_t nq, float* D, int64_t ldd, uint64_t* launches, int64_t form_nq = 0);
+
+// Collect mode of a filtered graph search (capi.cu).  collect_pass: the pass bitmap of rows [0, r.row_end) into
+// ix->s_cpass (not deleted, and passing r.d_prog at distance 0) and its popcount P; synchronises the stream to read P.
+int collect_pass(Index* ix, const ScanRequest& r, int64_t* P, uint64_t* launches);
+// passing_topk: the exact top-k over the P rows of that bitmap for the nb queries d_idx picks of the nq queries
+// (d_idx null: all of them, nb = nq), written over their rows of d_topk [nq x k].  Rows are compacted into an ascending
+// id list and scanned in chunks with the fp32 kernel of a batch of nq queries, so the keys are bitwise those of the
+// exact scan of rows [0, n_rows) with the same filter, in prefilter mode with the coarse pass off.  Synchronises the
+// stream when d_idx is set.
+int passing_topk(Index* ix, const float* queries, int64_t nq, const int* d_idx, int64_t nb, int64_t k, int64_t P,
+                 unsigned long long* d_topk, eps_stats* stats);
 
 // tc_dist.cu: wgmma TF32 / BF16 coarse distances (same contract as launch_distances, values carry ~1e-3 rel. error)
 bool tc_dist_usable(const Index* ix, int64_t nq);
@@ -306,8 +323,16 @@ int sparse_graph_search(Index* ix, const SparseQueries& q, int64_t nq, int64_t L
 // ---- graph_search.cu -----------------------------------------------------------------------
 // Best-first search of nq queries over the installed CSR graph with queue length L (<= n_indexed).
 // Output: d_queue [nq x L] sorted keys.
+// collect (a filtered search in EPS_FILTER_SEARCH_COLLECT): the same navigation, and per query the best `cap` keys of
+// the rows it evaluates whose bit is set in `pass` (rows [0, n_indexed) at least), into out [nq x cap], ascending,
+// kKeyInf padded.
+struct GraphCollect {
+  const uint32_t* pass;
+  unsigned long long* out;
+  int64_t cap;
+};
 int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsigned long long* d_queue,
-                 eps_stats* stats);
+                 eps_stats* stats, const GraphCollect* collect = nullptr);
 int prepare_init_ids(Index* ix, int64_t L);
 // Launch prologue shared by graph_search and sparse_graph_search: L in [1, n_indexed] (`who` names the caller in the
 // error), the padded queue length Lp (a power of two >= 2, at most 16384) and the init ids.
@@ -357,6 +382,12 @@ int finalize_graph(Index* ix, unsigned long long* d_queue, int64_t nq, int64_t L
 // Brute-force results: first min(valid, limit_cap) keys -> ids/dists/counts.
 int finalize_keys(Index* ix, const unsigned long long* d_topk, int64_t nq, int64_t k, int64_t limit, int64_t cap,
                   int64_t* d_ids, float* d_dists, int64_t* d_counts);
+// Collect mode: per query, the first cap keys of the merge of the graph search's passing-row list [nq x cap] and the
+// tail scan's top keys [nq x tail_k] (disjoint rows; tail may be null) into out [nq x cap]; the queries left with fewer
+// than min(cap, P) keys are listed on the device at *d_short_idx (in ix->s_cshort), and their number goes to *n_short
+// (synchronises the stream).
+int collect_merge(Index* ix, const unsigned long long* d_list, const unsigned long long* d_tail, int64_t nq, int64_t cap,
+                  int64_t tail_k, int64_t P, unsigned long long* d_out, const int** d_short_idx, int64_t* n_short);
 // shard s reads ids + s*id_stride and dists + s*dist_stride (elements; <= 0: the dense [n_shards x nq x k] layout)
 int merge_shards(int device, cudaStream_t stream, const int64_t* d_ids, const float* d_dists, int64_t n_shards,
                  int64_t nq, int64_t k, int64_t* d_out_ids, float* d_out_dists, int64_t id_stride = 0,

@@ -5,6 +5,7 @@ import numpy as np
 
 from .lib import BuildParams, FacetSpec, FilterNode, StatsStruct, check, load_library
 
+FILTER_SEARCH_MODES = {"post": 0, "collect": 1}
 METRICS = {"l2": 1, "euclidean": 1, "cosine": 2, "cos": 2, "ip": 3, "dot": 3, "dot_product": 3}
 
 
@@ -144,6 +145,13 @@ class Index:
     def set_search_width(self, width):
         """1 = sequential expansion order of the reference (IntraQueryThreads=1); 2/4 = parallel expansion."""
         check(self.L.eps_index_set_search_width(self.h, int(width)))
+
+    def set_filter_search(self, mode):
+        """Graph branch of a filtered search (eps_index_set_filter_search): "post" (default) = the reference's
+        post-filter of the unfiltered queue, which can return fewer than `limit` rows; "collect" = min(limit, L_local,
+        passing rows) rows per query, from the passing rows the graph search evaluates and an exact scan of the
+        passing rows for the queries it leaves short."""
+        check(self.L.eps_index_set_filter_search(self.h, FILTER_SEARCH_MODES.get(mode, mode)))
 
     def set_graph_tuning(self, ring_slots=0, ctas_per_sm=0):
         """Launch geometry of the graph kernel (0 = auto): TMA row-ring slots per CTA, resident CTAs per SM."""

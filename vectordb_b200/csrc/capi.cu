@@ -474,7 +474,11 @@ int eps_index_create(eps_index** out, int metric, int64_t dim, const float* host
   ix->capacity = capacity_rows;
   ix->host_vectors = host_vectors;
   cudaDeviceProp prop;
-  if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) ix->num_sms = prop.multiProcessorCount;
+  if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) {
+    ix->num_sms = prop.multiProcessorCount;
+    ix->smem_per_sm = static_cast<int>(prop.sharedMemPerMultiprocessor);
+    ix->smem_reserved_per_cta = static_cast<int>(prop.reservedSharedMemPerBlock);
+  }
   cudaError_t e = cudaStreamCreateWithFlags(&ix->stream, cudaStreamNonBlocking);
   if (e != cudaSuccess) return eps::fail(EPS_ERR_CUDA, cudaGetErrorString(e));
   for (auto& ev : ix->ev) cudaEventCreate(&ev);
@@ -545,7 +549,7 @@ int eps_index_create_view(eps_index* base_h, eps_index** out) {
   Index* ix = new Index();
   ix->view_of = base;
   ix->device = base->device; ix->metric = base->metric; ix->dim = base->dim; ix->sparse = base->sparse;
-  ix->num_sms = base->num_sms;
+  ix->num_sms = base->num_sms; ix->smem_per_sm = base->smem_per_sm; ix->smem_reserved_per_cta = base->smem_reserved_per_cta;
   static_cast<eps::Table&>(*ix) = *base;
   static_cast<eps::Config&>(*ix) = *base;
   cudaError_t e = cudaStreamCreateWithFlags(&ix->stream, cudaStreamNonBlocking);

@@ -63,9 +63,9 @@ constexpr int kMaxS = 8;        // ring slots per consumer warp (upper bound)
 constexpr int kMaxR = 24;       // ring slots (upper bound: 3 consumer warps x kMaxS)
 constexpr int kRounds = kMaxW * kEll / kGsThreads;  // adjacency slots per thread
 
-// Developer build only (make EXTRA=-DEPS_GS_PROFILE): per-phase cycle counters of warp 0 (pick / adjacency / merge /
-// barrier waits) and of warp 1 (row wait / row math), summed over CTAs into the kGcPhase slots of the counter block, the
-// visited-set counts and a per-query timeline.  Compiled out otherwise.
+// Developer build only (make EXTRA=-DEPS_GS_PROFILE): per-phase cycle counters of warp 0 (pick / adjacency / screen /
+// merge / barrier waits) and of warp 1 (row wait + math), summed over CTAs into the kGcPhase slots of the counter block,
+// the visited-set counts and a per-query timeline.  Compiled out otherwise.
 #ifdef EPS_GS_PROFILE
 #define GS_T(var) const long long var = clock64()
 #define GS_ACC(slot, t0, t1) do { if (lane == 0) prof[slot] += (t1) - (t0); } while (0)
@@ -317,7 +317,7 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
   const int n_own = cw >= 0 ? (R - cw + 2) / 3 : 0;  // slots cw, cw + 3, ... < R
   unsigned long long st_ndist = 0, st_nexp = 0, st_nedge = 0, st_nscr = 0;
 #ifdef EPS_GS_PROFILE
-  long long prof[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // 0 barrier X, 1 merge, 2 row wait, 3 row math, 4 pick, 5 barrier 1, 6 adjacency+visited, 7 barrier 2 + FIFO
+  long long prof[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // 0 barrier X, 1 merge, 2 screen, 3 row wait + math, 4 pick, 5 barrier 1, 6 adjacency+visited, 7 barrier 2 + FIFO
   const long long t_kernel0 = clock64();
   unsigned long long prof_vtest = 0, prof_migrated = 0;  // hash-set test-and-inserts of this thread; queries moved to the bitmap
 #endif
@@ -655,6 +655,7 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
         }
       }
       if (kScreen) fresh_n += static_cast<uint32_t>(total);
+      GS_T(ts0);
       // -- A2: screen the fresh ids on their sketches once the queue holds L entries (block-uniform) --
       const unsigned long long sbound = kScreen ? qa[L - 1] & kKeyMask : kKeyInf;
       if (kScreen && total > 0 && sbound != kKeyInf) {
@@ -683,6 +684,8 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
       } else {
         fifo_tail += static_cast<uint32_t>(total);
       }
+      GS_T(ts1);
+      GS_ACC(2, ts0, ts1);
       if (cont_mode) {
         if (tid == 0) {
           s_cont_e[ncont - 1] = e0 + nslots;
@@ -708,6 +711,7 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
       if (tid == 0) st_ndist += static_cast<unsigned long long>(total);
       GS_T(tf1);
       GS_ACC(7, ta1, tf1);
+      GS_ACC(7, ts1, ts0);  // less the screen, which is its own phase
     }
 
     // ---- results + visited reset (:711-714) ----
@@ -894,16 +898,33 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   // partly filled last wave is pure loss while the kernel is latency-bound; so among ring sizes >= 4 take the one
   // with the fewest rounds (a smaller ring = more resident queries), the largest ring on ties, and launch exactly
   // ceil(nq / rounds) CTAs so that every CTA serves the same number of queries (profiles/r02_graph_geometry_*).
+  // With the screen, between two rings with the same rounds and the same CTAs per SM (so the same kernel instance), one
+  // whose resident CTAs fit the 196 KB shared-memory carve-out wins over a larger one that needs the 228 KB carve-out,
+  // and the launch asks for that carve-out: it leaves the L1 60 KB of the SM's 256 KB instead of 28.  The screen's
+  // sketch loads keep up to 64 lines of 128 B in flight per CTA, 32 KB at 4 CTAs per SM.  On one H100 at 10M x 768,
+  // L = 768, 3 batches in flight, ring 10 at 4 CTAs per SM is 3 % faster than ring 12, and no faster with the carve-out
+  // pinned at 228 KB.  Without the screen (the clustered table, L = 1536) the smaller L1 costs nothing and a smaller
+  // ring does (ring 7 instead of 10: 1.5 %), so there the largest ring still wins.
+  constexpr size_t kL1Carveout = 196 * 1024;  // H100: the largest carve-out below the 228 KB maximum
+  if (screen && ix->gs_static_smem < 0) {
+    cudaFuncAttributes fa;
+    EPS_CUDA(cudaFuncGetAttributes(&fa, kernels[ci][1][1]));
+    ix->gs_static_smem = static_cast<int>(fa.sharedSizeBytes);
+  }
+  auto sm_smem = [&](int r, int p) { return static_cast<size_t>(p) * (smem_for(r) + ix->gs_static_smem + ix->smem_reserved_per_cta); };
+  auto l1_kept = [&](int r, int p) { return screen && sm_smem(r, p) <= kL1Carveout; };
   auto rounds_of = [&](int p) { return (nq + static_cast<int64_t>(p) * ix->num_sms - 1) / (static_cast<int64_t>(p) * ix->num_sms); };
+  bool keep_l1 = false;
   if (staged && ix->graph_ring_slots == 0 && rounds_of(per_sm) > 1) {
     int best_r = R, best_p = per_sm;
     for (int r = R - 1; r >= 4; --r) {
       int p = 0;
       EPS_TRY(resident(r, &p));
-      if (rounds_of(p) < rounds_of(best_p)) { best_r = r; best_p = p; }
+      if (rounds_of(p) < rounds_of(best_p) || (p == best_p && l1_kept(r, p) && !l1_kept(best_r, best_p))) { best_r = r; best_p = p; }
     }
     R = best_r;
     per_sm = best_p;
+    keep_l1 = l1_kept(R, per_sm);
   }
   const size_t smem = smem_for(R);
   const int64_t rounds = rounds_of(per_sm);
@@ -965,7 +986,13 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   // at most 4 resident CTAs per SM (what the auto rule picks for batches above one wave at 7 per SM, e.g. 1024 queries
   // at L = 768): the register file has room for 128 registers per thread, so the instance that hardly spills runs;
   // smaller batches keep 7 resident queries per SM
-  kernels[ci][per_sm <= 4 ? 1 : 0][screen ? 1 : 0]<<<slots, kGsThreads, smem, ix->stream>>>(a);
+  const Kernel kernel = kernels[ci][per_sm <= 4 ? 1 : 0][screen ? 1 : 0];
+  // the smallest carve-out that holds the resident CTAs (the driver rounds the percentage up to one it supports), or
+  // the driver's own choice
+  const int carveout = keep_l1 ? static_cast<int>((100 * sm_smem(R, per_sm) + ix->smem_per_sm - 1) / ix->smem_per_sm)
+                               : static_cast<int>(cudaSharedmemCarveoutDefault);
+  EPS_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carveout));
+  kernel<<<slots, kGsThreads, smem, ix->stream>>>(a);
   EPS_CUDA(cudaGetLastError());
   if (stats) {
     stats->n_seed += static_cast<uint64_t>(nq) * static_cast<uint64_t>(L);
@@ -1033,7 +1060,7 @@ int read_graph_counters(Index* ix, eps_stats* stats) {
   stats->n_edges += h[kGcEdges];
 #ifdef EPS_GS_PROFILE
   const unsigned long long* pr = h;
-  const char* names[8] = {"barrierX", "merge", "row_wait", "team_phase", "pick", "barrier1", "adj+visited", "barrier2+fifo"};
+  const char* names[8] = {"barrierX", "merge", "screen", "rows", "pick", "barrier1", "adj+visited", "barrier2+fifo"};
   const double tot = static_cast<double>(pr[kGcCycles]) + 1.0;
   fprintf(stderr, "[gs-profile] kernel cycles summed over CTAs %.3e;", tot);
   for (int w = 0; w < 2; ++w)

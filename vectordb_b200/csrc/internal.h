@@ -148,6 +148,9 @@ struct Index : Table, Config {
   int64_t dim = 0;
   bool sparse = false;
   int num_sms = 132;
+  int smem_per_sm = 228 * 1024;   // shared memory an SM can give its CTAs (the largest carve-out)
+  int smem_reserved_per_cta = 1024;  // shared memory the driver reserves per resident CTA
+  int gs_static_smem = -1;        // static shared memory of the screened graph kernel (-1: not read yet)
   const float* host_vectors = nullptr;
   Index* view_of = nullptr;     // read-only view (eps_index_create_view): its Table belongs to this index
   int n_views = 0;              // live views of this index; mutating entry points refuse while > 0

@@ -241,22 +241,22 @@ EPS_API int eps_index_set_filter_search(eps_index* ix, int mode);
  * (0 = whatever fits).  No reference counterpart (the CPU executor has no such geometry). */
 EPS_API int eps_index_set_graph_tuning(eps_index* ix, int ring_slots, int ctas_per_sm);
 
-/* Graph-search screen (L2 only; never changes results).  When a graph is installed (eps_index_build,
+/* Graph-search screen (L2, inner product and cosine; never changes results).  When a graph is installed (eps_index_build,
  * eps_index_set_graph), the index computes the top-32 principal subspace P~ of its rows (covariance of up to 2^20 rows,
  * subspace iteration in double) and, when the screen is on, a 32-float sketch fl(P~(x - mu)) of every indexed row with
- * a bound on its rounding error: 132 bytes per row next to the row's 4 * dim.  The search then reads the sketch of a
- * fresh neighbour first and fetches its row only when a proven lower bound on its distance, taken from the sketches,
- * cannot reject it (DESIGN.md §K2); ids, distances and all eps_stats counters are those of the unscreened search.
+ * a bound on its rounding error: 132 bytes per row next to the row's 4 * dim (140 for inner product and cosine, which
+ * also keep the norm of the row's residual outside the subspace and its product with the mean).  The search then reads
+ * the sketch of a fresh neighbour first and fetches its row only when a proven lower bound on its distance, taken from
+ * the sketches, cannot reject it (DESIGN.md §K2; for inner product and cosine, from an upper bound on the fp32 dot
+ * product); ids, distances and all eps_stats counters are those of the unscreened search.
  * mode: EPS_GRAPH_SCREEN_OFF, _ON, or _AUTO (default): on when the 32 components carry at least 90 % of the sampled
- * variance, i.e. when the rows lie close to a low-dimensional subspace.  Tables below 128 dimensions are not screened.
- * Inner-product and cosine indexes are not screened: their bound would also need the norm of each row's residual
- * outside the subspace. */
+ * variance, i.e. when the rows lie close to a low-dimensional subspace.  Tables below 128 dimensions are not screened. */
 #define EPS_GRAPH_SCREEN_OFF 0
 #define EPS_GRAPH_SCREEN_ON 1
 #define EPS_GRAPH_SCREEN_AUTO 2
 EPS_API int eps_index_set_graph_screen(eps_index* ix, int mode);
 /* State of the screen: active = whether the next graph search screens, share = share of the sampled variance the
- * basis carries (-1 when no basis was computed: no graph, not L2, below 128 dimensions, or mode off since the install),
+ * basis carries (-1 when no basis was computed: no graph, below 128 dimensions, or mode off since the install),
  * n_screened = fresh neighbours dropped by the screen in all graph searches of this handle so far, with or without a
  * stats argument (waits for the handle's stream).  The count is kept here rather than in eps_stats so that eps_stats
  * keeps its size and layout.  The sketch is computed when a graph is installed and when this mode changes, never

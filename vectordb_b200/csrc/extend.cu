@@ -355,15 +355,21 @@ int extend_repair(Index* ix, const eps_build_params& bp, Phases* ph) {
   return upload_csr(ix, n, off2.data(), nb2.data(), off2[n], nav);
 }
 
-// Stored row sketches of [0, n0) extended to [0, n_indexed) with the kept basis: [n x m] sketches, then [n] bounds.
+// Stored row sketches of [0, n0) extended to [0, n_indexed) with the kept basis: [n x m] sketches, then [n] bounds,
+// then (inner product, cosine) [n] dot-product terms.
 int extend_sketches(Index* ix, int64_t n0) {
   const int64_t n = ix->n_indexed, m = ix->sk_m;
   Mem fresh;
-  EPS_TRY(fresh.reserve(static_cast<size_t>(n) * (m + 1) * 4));
+  EPS_TRY(fresh.reserve(static_cast<size_t>(sketch_floats(ix, n)) * 4));
   float* sk = fresh.as<float>();
   EPS_CUDA(cudaMemcpyAsync(sk, ix->d_sk, static_cast<size_t>(n0) * m * 4, cudaMemcpyDeviceToDevice, ix->stream));
   EPS_CUDA(cudaMemcpyAsync(sk + n * m, ix->d_sk + n0 * m, static_cast<size_t>(n0) * 4, cudaMemcpyDeviceToDevice, ix->stream));
   EPS_TRY(sketch_rows(ix, ix->d_vectors + n0 * ix->dim, n - n0, sk + n0 * m, sk + n * m + n0));
+  if (ix->metric != EPS_METRIC_L2) {
+    float2* terms = reinterpret_cast<float2*>(sk + sk_terms_off(n));
+    EPS_CUDA(cudaMemcpyAsync(terms, ix->d_sk + sk_terms_off(n0), static_cast<size_t>(n0) * 8, cudaMemcpyDeviceToDevice, ix->stream));
+    EPS_TRY(dot_row_terms(ix, ix->d_vectors + n0 * ix->dim, n - n0, terms + n0));
+  }
   EPS_CUDA(cudaStreamSynchronize(ix->stream));
   ix->d_sk.swap(fresh);
   return EPS_OK;

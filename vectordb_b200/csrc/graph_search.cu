@@ -34,8 +34,9 @@
 //     query that would fill the set beyond 3/4 moves to a bitmap of n bits (atomicOr test-and-set) for the rest of
 //     its run; that bitmap is cleared after the query — on large tables only the words the query touched, from a log
 //     of its fresh ids.
-//   * screen (L2, sketch.cu): once the queue holds L entries, the fresh ids of a step are checked against a proven lower
-//     bound from 32-float principal-subspace sketches of the row and the query, and only those it cannot reject enter
+//   * screen (sketch.cu; L2, and inner product / cosine through a bound on the dot product): once the queue holds L
+//     entries, the fresh ids of a step are checked against a proven lower bound from 32-float principal-subspace
+//     sketches of the row and the query, and only those it cannot reject enter
 //     the FIFO and have their rows fetched (screen_fresh; DESIGN.md §K2);
 // every iteration picks up to W (the search width) unchecked candidates, and the next pick waits until all their rows
 //   are consumed and merged.  The result at any width W is that of this rule: each step takes the first
@@ -174,49 +175,89 @@ __device__ __forceinline__ void warp_rows_scalar(const float* const (&rows)[S], 
 // make_key(LB, id) >= bound; the consumer's bound is at most this one, so it would have dropped the id too.  Bit i of
 // keep is set for every id i that stays.  In collect mode the id must also stay out of the passing rows' list: it is
 // dropped only when it fails the filter or make_key(LB, id) >= rbound, the list's worst key (kKeyInf until it is full).
+//
+// Inner product and cosine (kScreenDot): the consumer computes acc = the fp32 dot product of q and x (lane fmaf chains
+// of at most 4 ceil(d / 128) terms, then the 5-step butterfly: n_c = 4 ceil(d / 128) + 5 roundings, which also covers
+// the scalar path's ceil(d / 32) + 5) and the distance base - acc (IP: -acc, base = 0; cosine: fl(1 - acc)).  With
+// y = x - mu, q' = q - mu and A = I - P~^T P~ (symmetric, A - A^2 = P~^T (I - P~ P~^T) P~, so |A - A^2| <= eps (1 + eps)):
+//   <q, x> = <q, mu> + <mu, y> + <P~ q', P~ y> + <A q', A y> + q'^T (A - A^2) y
+//   acc    <= <q, x> + gamma_{n_c} |q| |x| + n_c 2^-149                         (n_c 2^-149: products that underflow)
+// and, with the sketches s^_x (bound ex_x) and p^_q (bound E_q) and s^ = the 8-lane fp32 sum of their products (lane
+// chains of 4, 3-step butterfly: error <= gamma_7 |p^_q| |s^_x| + 7 2^-149),
+//   <P~ q', P~ y> <= s^ + gamma_7 |p^_q| |s^_x| + E_q |s^_x| + |p^_q| ex_x + E_q ex_x + 7 2^-149.
+// Each row's ex_x bounds its |y| (|y| <= k ex_x, k = 1 / (sqrt(m) gamma_{d+2} sqrt(1 + eps)), see sketch_rows_kernel),
+// and so |s^_x| <= (sqrt(1 + eps) k + 1) ex_x and |x| <= |mu| + k ex_x.  That folds every query-only factor into four
+// numbers per query, computed in double and rounded up by dot_terms_kernel (sketch.cu), psk[kSketch ..]:
+//   UB = s^ + (C0 - base) + <mu, y> + |A q'| |A y| + C_ex ex_x,   every step rounded up (__fadd_ru, __fmul_ru);
+//   LB = -0 - UB rounded down  (= round_down(base - UB): IP -UB, cosine round_down(1 - UB); -0 for a zero)
+// with <mu, y> and |A y| stored per row (float2, rounded up).  acc <= UB, and base - acc and fl(1 - acc) are
+// non-increasing in acc, so LB never exceeds the consumer's distance.  The consumer's products and partial sums stay
+// below FLT_MAX when |q| |x| < 2^126: an id is dropped only when K ex_x < 2^125 (K = |q| k; +inf when |q| |mu| >= 2^125),
+// UB is finite (NaN or inf from any term, a row that overflows, a query whose norm is not finite: kept), and
+// make_key(LB, id) >= bound, with the same collect-mode condition as L2.
 constexpr int kScreenIds = 64;  // ids whose loads are in flight together (4 per 8-lane group)
-template <bool kCollect>
+template <int kScreen, bool kCollect>
 __device__ __forceinline__ void screen_fresh(const GSArgs& a, const int* fifo, unsigned fmask, uint32_t tail, int total, const float* psk,
                                              unsigned long long bound, unsigned long long rbound, int tid, unsigned* keep) {
+  constexpr bool kDot = kScreen == kScreenDot;
   const int g = tid >> 3, j = tid & 7;
   constexpr int kPer = kScreenIds / (kGsThreads / 8);
   const float4* sk4 = reinterpret_cast<const float4*>(a.sk);
   const float* skex = a.sk + a.n_sk * kSketch;
+  const float2* skt = kDot ? reinterpret_cast<const float2*>(a.sk + sk_terms_off(a.n_sk)) : nullptr;
   const float4 p0 = reinterpret_cast<const float4*>(psk)[j];
   const float eq = psk[kSketch];
+  const float4 qc = kDot ? reinterpret_cast<const float4*>(psk + kSketch)[0] : make_float4(0.f, 0.f, 0.f, 0.f);  // C0 - base, C_ex, |A q'|, K
   for (int i0 = 0; i0 < total; i0 += kScreenIds) {
     int id[kPer];
     float4 x0[kPer];
     float xe[kPer];
+    float2 xt[kPer];
 #pragma unroll
     for (int b = 0; b < kPer; ++b) {
       const int i = i0 + b * (kGsThreads / 8) + g;
       id[b] = i < total ? fifo[(tail + static_cast<uint32_t>(i)) & fmask] : -1;
       x0[b] = p0;
       xe[b] = 0.f;
+      if (kDot) xt[b] = make_float2(0.f, 0.f);
       if (id[b] >= 0) {
         x0[b] = __ldg(sk4 + static_cast<int64_t>(id[b]) * (kSketch / 4) + j);
         if (j == 0) xe[b] = __ldg(skex + id[b]);
+        if (kDot && j == 0) xt[b] = __ldg(skt + id[b]);
       }
     }
 #pragma unroll
     for (int b = 0; b < kPer; ++b) {
       float acc = 0.f, d;
-      d = x0[b].x - p0.x; acc = fmaf(d, d, acc); d = x0[b].y - p0.y; acc = fmaf(d, d, acc);
-      d = x0[b].z - p0.z; acc = fmaf(d, d, acc); d = x0[b].w - p0.w; acc = fmaf(d, d, acc);
+      if (kDot) {
+        acc = fmaf(x0[b].x, p0.x, acc); acc = fmaf(x0[b].y, p0.y, acc); acc = fmaf(x0[b].z, p0.z, acc); acc = fmaf(x0[b].w, p0.w, acc);
+      } else {
+        d = x0[b].x - p0.x; acc = fmaf(d, d, acc); d = x0[b].y - p0.y; acc = fmaf(d, d, acc);
+        d = x0[b].z - p0.z; acc = fmaf(d, d, acc); d = x0[b].w - p0.w; acc = fmaf(d, d, acc);
+      }
       acc += __shfl_xor_sync(kFull, acc, 1);
       acc += __shfl_xor_sync(kFull, acc, 2);
       acc += __shfl_xor_sync(kFull, acc, 4);
       if (j == 0 && id[b] >= 0) {
         const int i = i0 + b * (kGsThreads / 8) + g;
-        float r = __fsqrt_rd(__fmul_rd(acc, a.sk_g));
-        r = __fsub_rd(__fsub_rd(r, xe[b]), eq);
         bool drop = false;
-        if (r > 0.f) {  // false for NaN as well
-          const float lb = __fmul_rd(__fmul_rd(r, r), a.sk_scale);
-          drop = lb <= FLT_MAX && make_key(lb, static_cast<uint32_t>(id[b])) >= bound;
+        if (kDot) {
+          float ub = __fadd_ru(__fadd_ru(acc, qc.x), xt[b].y);
+          ub = __fadd_ru(ub, __fmul_ru(qc.z, xt[b].x));
+          ub = __fadd_ru(ub, __fmul_ru(qc.y, xe[b]));
+          const float lb = __fsub_rd(-0.f, ub);
+          drop = __fmul_ru(qc.w, xe[b]) < 0x1.0p125f && fabsf(ub) <= FLT_MAX && make_key(lb, static_cast<uint32_t>(id[b])) >= bound;
           if (kCollect && drop)
             drop = !row_passes(a.pass, static_cast<uint32_t>(id[b])) || make_key(lb, static_cast<uint32_t>(id[b])) >= rbound;
+        } else {
+          float r = __fsqrt_rd(__fmul_rd(acc, a.sk_g));
+          r = __fsub_rd(__fsub_rd(r, xe[b]), eq);
+          if (r > 0.f) {  // false for NaN as well
+            const float lb = __fmul_rd(__fmul_rd(r, r), a.sk_scale);
+            drop = lb <= FLT_MAX && make_key(lb, static_cast<uint32_t>(id[b])) >= bound;
+            if (kCollect && drop)
+              drop = !row_passes(a.pass, static_cast<uint32_t>(id[b])) || make_key(lb, static_cast<uint32_t>(id[b])) >= rbound;
+          }
         }
         if (!drop) atomicOr(keep + (i >> 5), 1u << (i & 31));
       }
@@ -261,11 +302,12 @@ __device__ __forceinline__ void consume_slots(const GSArgs& a, unsigned occ_mask
 
 // Two register budgets of the same kernel: 72 registers per thread allow 7 resident CTAs per SM but spill 376 B per
 // thread to local memory (348 B of spill loads); 128 registers allow 4 and spill 12 B (16 B of loads).  graph_search
-// picks the instance from the geometry it launches.  kScreen: the screen is compiled in only where it runs, so that a
-// search without it (other metrics, tables it cannot pay on) keeps the registers of the kernel without it.  kCollect: the
+// picks the instance from the geometry it launches.  kScreen: the screen kind (kScreenNone, kScreenL2, kScreenDot for
+// inner product and cosine) is compiled in only where it runs, so that a search without it (tables it cannot pay on)
+// keeps the registers of the kernel without it, and the L2 instances carry no metric branch.  kCollect: the
 // collect mode of a filtered search (DESIGN.md §K2), which navigates as the other instances do and also keeps each
 // query's list of the best a.cap keys of the passing rows it evaluates, merged like the queue.
-template <int kMinCtas, bool kScreen, bool kCollect = false>
+template <int kMinCtas, int kScreen, bool kCollect = false>
 __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSArgs a) {
   extern __shared__ __align__(128) unsigned char gs_smem[];
   const int dim4p = (a.dim + 3) & ~3;
@@ -337,8 +379,11 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
     // ---- seed (InitializeSetLPara): precomputed distances of the query-independent seed set ----
     for (int i = tid; i < a.dim; i += kGsThreads) qv[i] = a.queries[static_cast<int64_t>(q) * a.dim + i];
     for (int i = a.dim + tid; i < dim4p; i += kGsThreads) qv[i] = 0.f;
-    if (kScreen && tid <= kSketch)
+    if (kScreen == kScreenL2 && tid <= kSketch)
       psk[tid] = tid < kSketch ? a.qsk[static_cast<int64_t>(q) * kSketch + tid] : a.qsk[static_cast<int64_t>(a.nq) * kSketch + q];
+    if (kScreen == kScreenDot && tid < kSketch + 4)  // the sketch, then C0 - base, C_ex, |A q'|, K
+      psk[tid] = tid < kSketch ? a.qsk[static_cast<int64_t>(q) * kSketch + tid]
+                               : a.qsk[sk_qterms_off(a.nq) + 4 * static_cast<int64_t>(q) + tid - kSketch];
     bool hashed = L <= a.vset_max;  // the visited set is the hash set (false: the query has moved to the bitmap)
     for (int i = tid; i < a.Lp; i += kGsThreads) {
       unsigned long long key = kKeyInf;
@@ -660,7 +705,7 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
       const unsigned long long sbound = kScreen ? qa[L - 1] & kKeyMask : kKeyInf;
       if (kScreen && total > 0 && sbound != kKeyInf) {
         __syncthreads();  // (3) the fresh ids are in the FIFO, s_keep is clear
-        screen_fresh<kCollect>(a, fifo, fmask, fifo_tail, total, psk, sbound, kCollect ? rq[a.cap - 1] : kKeyInf, tid, s_keep);
+        screen_fresh<kScreen, kCollect>(a, fifo, fmask, fifo_tail, total, psk, sbound, kCollect ? rq[a.cap - 1] : kKeyInf, tid, s_keep);
         int mine[kMaxW * kEll / kGsThreads];
 #pragma unroll
         for (int r = 0; r < kMaxW * kEll / kGsThreads; ++r) {
@@ -866,7 +911,7 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   int R = ring_slots_for(ix, slot_bytes);
   // FIFO: a backlog below R entries + the ids one A step appends (W adjacency rows or one 128-id continuation chunk)
   const int fc = next_pow2(std::max(width * kEll, kGsThreads) + kMaxR);
-  const bool screen = screen_on(ix);  // the query sketch takes shared memory only when the screen runs
+  const int screen = screen_kind(ix);  // the query sketch takes shared memory only when the screen runs
   // collect: the passing rows' list and its pending keys after the bitmap words (padded to an even count)
   const size_t collect_bytes = collect ? 4 + static_cast<size_t>(collect->cap + kPC) * 8 : 0;
   auto smem_for = [&](int r) {
@@ -877,14 +922,15 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   while (R > 2 && smem_for(R) > 200 * 1024) --R;
   if (smem_for(R) > 226 * 1024) return fail(EPS_ERR_UNSUPPORTED, "queue + query + row ring do not fit in shared memory");
   using Kernel = void (*)(GSArgs);
-  // [collect][per_sm <= 4][screen]
-  const Kernel kernels[2][2][2] = {{{graph_search_kernel<7, false>, graph_search_kernel<7, true>},
-                                    {graph_search_kernel<4, false>, graph_search_kernel<4, true>}},
-                                   {{graph_search_kernel<7, false, true>, graph_search_kernel<7, true, true>},
-                                    {graph_search_kernel<4, false, true>, graph_search_kernel<4, true, true>}}};
+  // [collect][per_sm <= 4][screen kind]
+  const Kernel kernels[2][2][3] = {
+      {{graph_search_kernel<7, kScreenNone>, graph_search_kernel<7, kScreenL2>, graph_search_kernel<7, kScreenDot>},
+       {graph_search_kernel<4, kScreenNone>, graph_search_kernel<4, kScreenL2>, graph_search_kernel<4, kScreenDot>}},
+      {{graph_search_kernel<7, kScreenNone, true>, graph_search_kernel<7, kScreenL2, true>, graph_search_kernel<7, kScreenDot, true>},
+       {graph_search_kernel<4, kScreenNone, true>, graph_search_kernel<4, kScreenL2, true>, graph_search_kernel<4, kScreenDot, true>}}};
   const int ci = collect ? 1 : 0;
   for (int p = 0; p < 2; ++p)
-    for (int s = 0; s < 2; ++s)
+    for (int s = 0; s < 3; ++s)
       EPS_CUDA(cudaFuncSetAttribute(kernels[ci][p][s], cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem_for(R))));
   auto resident = [&](int r, int* out) {
     EPS_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(out, kernels[ci][0][0], kGsThreads, smem_for(r)));
@@ -908,7 +954,7 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   constexpr size_t kL1Carveout = 196 * 1024;  // H100: the largest carve-out below the 228 KB maximum
   if (screen && ix->gs_static_smem < 0) {
     cudaFuncAttributes fa;
-    EPS_CUDA(cudaFuncGetAttributes(&fa, kernels[ci][1][1]));
+    EPS_CUDA(cudaFuncGetAttributes(&fa, kernels[ci][1][screen]));
     ix->gs_static_smem = static_cast<int>(fa.sharedSizeBytes);
   }
   auto sm_smem = [&](int r, int p) { return static_cast<size_t>(p) * (smem_for(r) + ix->gs_static_smem + ix->smem_reserved_per_cta); };
@@ -970,10 +1016,9 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
       EPS_TRY(ix->d_screened.reserve(8));
       EPS_CUDA(cudaMemsetAsync(ix->d_screened, 0, 8, ix->stream));
     }
-    EPS_TRY(ix->s_qsk.reserve(static_cast<size_t>(nq) * (kSketch + 1) * 4));
+    EPS_TRY(ix->s_qsk.reserve(static_cast<size_t>(sketch_query_floats(screen, nq)) * 4));
     float* qsk = ix->s_qsk.as<float>();
-    EPS_TRY(sketch_rows(ix, d_queries, nq, qsk, qsk + nq * kSketch));
-    ++launches;
+    EPS_TRY(sketch_queries(ix, d_queries, nq, qsk, &launches));
     a.sk = ix->d_sk; a.qsk = qsk; a.n_sk = ix->n_indexed; a.sk_g = ix->sk_g; a.sk_scale = ix->sk_scale;
     a.n_screened = ix->d_screened;
   }
@@ -986,7 +1031,7 @@ int graph_search(Index* ix, const float* d_queries, int64_t nq, int64_t L, unsig
   // at most 4 resident CTAs per SM (what the auto rule picks for batches above one wave at 7 per SM, e.g. 1024 queries
   // at L = 768): the register file has room for 128 registers per thread, so the instance that hardly spills runs;
   // smaller batches keep 7 resident queries per SM
-  const Kernel kernel = kernels[ci][per_sm <= 4 ? 1 : 0][screen ? 1 : 0];
+  const Kernel kernel = kernels[ci][per_sm <= 4 ? 1 : 0][screen];
   // the smallest carve-out that holds the resident CTAs (the driver rounds the percentage up to one it supports), or
   // the driver's own choice
   const int carveout = keep_l1 ? static_cast<int>((100 * sm_smem(R, per_sm) + ix->smem_per_sm - 1) / ix->smem_per_sm)

@@ -121,8 +121,11 @@ struct Table {
   float sk_g = 0.f;              // 1 - gamma_{m+2}, rounded down
   float sk_scale = 0.f;          // (1 - 2 (dim + 2) 2^-24) / (1 + eps), rounded down
   double sk_eps = 0.0;           // sigma_max(P~)^2 <= 1 + sk_eps
+  double sk_mu_norm = 0.0;       // |mu|, rounded up
   DevArray<float> d_sk_basis;    // [dim x sk_m] fp32 basis P~ (transposed), then [dim] mean
-  DevArray<float> d_sk;          // [n_indexed x sk_m] row sketches, then [n_indexed] their error bounds (null: screen off)
+  // [n_indexed x sk_m] row sketches, then [n_indexed] their error bounds; inner product and cosine then add, from
+  // float sk_terms_off(n_indexed) on, [n_indexed] float2 {|A y|, <mu, y>} rounded up (null: screen off)
+  DevArray<float> d_sk;
 };
 
 // Executor and tuning parameters: a view starts with its base's and sets its own afterwards.
@@ -189,7 +192,7 @@ struct Index : Table, Config {
   int64_t prof_nq = 0;           // developer build (EPS_GS_PROFILE): queries of the last graph-search launch
   DevBuf s_prof_qtimes;          // developer build: [prof_nq x 4] per-query timeline of the last dense launch
   bool prof_timeline = false;    // developer build: s_prof_qtimes belongs to the last launch
-  DevBuf s_qsk;                  // [nq x sk_m] query sketches, then [nq] their error bounds
+  DevBuf s_qsk;                  // [nq x sk_m] query sketches, then [nq] their error bounds (+ dot-product terms, sketch_queries)
   DevArray<unsigned long long> d_screened;  // device count of the fresh neighbours the screen dropped on this handle
   DevArray<unsigned long long> d_l2_rescored;  // device count of the (query, row) pairs the L2 screen re-scored here
   HostBuf h_out;                 // pinned host mirror of the packed result block (eps_search_batch)
@@ -365,16 +368,29 @@ constexpr int kSketch = 32;       // floats per row sketch of the graph screen
 // Top-m principal subspace of the first n_indexed rows: basis [m x dim] row-major with orthonormal rows (the first k
 // rows span the top-k subspace), the sample mean [dim], and the share of the sample's variance the m rows carry.
 int principal_subspace(Index* ix, int m, std::vector<float>* basis, std::vector<float>* mean, double* share);
-// The graph search screens fresh neighbours with the sketch when the metric is L2 and the mode is on, or auto with the
-// basis carrying at least kScreenShare of the variance.
+// The graph search screens fresh neighbours with the sketch when the mode is on, or auto with the basis carrying at
+// least kScreenShare of the variance.  L2 bounds the distance; inner product and cosine bound the dot product.
 constexpr double kScreenShare = 0.9;
+constexpr int kScreenNone = 0, kScreenL2 = 1, kScreenDot = 2;  // the graph kernel's screen kinds
 // Basis (+ row sketches when the screen will run) of the installed graph's rows, at graph install and mode changes.
 // Never fails: a sketch that cannot be set up leaves the screen off.  Row sketches are freed when the screen is off.
 void ensure_sketch(Index* ix);
 void free_sketch(Index* ix);
 bool screen_on(const Index* ix);
+int screen_kind(const Index* ix);  // the kind the next graph search runs (kScreenNone when the screen is off)
+// float offset of the dot-product row terms in d_sk (8-byte aligned), and the floats d_sk takes, for n rows
+__host__ __device__ inline int64_t sk_terms_off(int64_t n) { return (n * (kSketch + 1) + 1) & ~static_cast<int64_t>(1); }
+int64_t sketch_floats(const Index* ix, int64_t n);
 // sketches and error bounds of n rows at d_x (the table's layout) with the index's basis
 int sketch_rows(Index* ix, const float* d_x, int64_t n, float* d_sk, float* d_ex);
+// dot-product screen: {|A y|, <mu, y>} of n rows at d_x, rounded up
+int dot_row_terms(Index* ix, const float* d_x, int64_t n, float2* d_terms);
+// the per-query block of a graph search's screen in qsk: [nq x kSketch] sketches of q - mu, [nq] their error bounds,
+// and for the dot-product kind, from float sk_qterms_off(nq) on (16-byte aligned for any nq), [nq x 4]
+// {C0, C_ex, |A (q - mu)|, K} (sketch.cu); returns the launches it took
+int sketch_queries(Index* ix, const float* d_q, int64_t nq, float* qsk, uint64_t* launches);
+__host__ __device__ inline int64_t sk_qterms_off(int64_t nq) { return (nq * (kSketch + 1) + 3) & ~static_cast<int64_t>(3); }
+inline int64_t sketch_query_floats(int kind, int64_t nq) { return kind == kScreenDot ? sk_qterms_off(nq) + 4 * nq : nq * (kSketch + 1); }
 
 // ---- finalize.cu ---------------------------------------------------------------------------
 // Post-filter walk / tail merge of VecSearchExecutor::Search (vec_search_executor.cpp:885-927).

@@ -1,8 +1,10 @@
-// Principal-subspace sketch of an L2 table (DESIGN.md §K2, "screen").
+// Principal-subspace sketch of a table (DESIGN.md §K2, "screen").
 //
 // For any matrix P with orthonormal rows, |P(x - q)|^2 <= |x - q|^2, so a projection of the rows onto the subspace that
 // carries most of their variance gives a cheap lower bound on a distance.  The graph search reads the m-float sketch
-// fl(P~(x - mu)) of a fresh neighbour and fetches its row only when that bound cannot reject it.
+// fl(P~(x - mu)) of a fresh neighbour and fetches its row only when that bound cannot reject it.  For inner product
+// and cosine the bound is an upper bound on the dot product, which also needs |A y| and <mu, y> of each row
+// (A = I - P~^T P~, y = x - mu) and a few numbers per query (dot_terms_kernel).
 //
 // Mean and covariance: two passes over up to 2^20 evenly spaced rows on the device, fp32 within a 512-row chunk and
 // fp64 across chunks.  Basis: block subspace iteration with modified Gram-Schmidt on the host in double (the library
@@ -151,6 +153,131 @@ float round_down(double x) {
   return f;
 }
 
+// Constants of the dot-product bound (graph_search.cu, screen_fresh), in double.
+struct DotConsts {
+  double ay_rel;    // |A y| <= (|r^| (1 + (d + 8) 2^-52) + |y^| ay_rel) (1 + 2^-50), see dot_terms_kernel
+  double mu_norm;   // |mu|, rounded up
+  double k;         // |y| <= k ex_x (ex_x = sqrt(m) (gamma_{d+2} sqrt(1 + eps) |y| + d 2^-149), rounded up)
+  double s1;        // sqrt(1 + eps) k + 1: |s^_x| <= s1 ex_x
+  double eps1;      // eps (1 + eps): |A - A^2| <= eps1
+  double g_c;       // gamma_{n_c}, n_c = 4 ceil(d / 128) + 5: the consumer's fp32 dot product (lane chains + butterfly)
+  double g7;        // gamma_7: the screen's 8-lane fp32 dot product of the sketches (4-step chains + 3-step butterfly)
+  double tiny;      // (n_c + 8) 2^-149: products and sums of both that underflow
+  double base;      // the metric's finish: distance = base - dot (IP: 0, cosine: 1)
+};
+
+// One warp per vector v, in double from the fp32 inputs: y = v - mu (each difference rounded once), w = P~ y (lane
+// chains + butterfly), r = y - P~^T w (a chain of m fma from y_k), and |y|^2, |r|^2, <mu, y>.  |r - A y| is bounded by
+// |y| (1 + eps) [gamma_m (1 + 1.01 sqrt(m)) + m gamma_{d+5}] (|P~|_F <= sqrt(m (1 + eps)), |w - P~ y| <= sqrt(m)
+// gamma_{d+5} sqrt(1 + eps) |y|), and |A| <= max(1, eps) carries the rounding of y; ay_rel holds both with a factor 2.
+// A row writes {|A y|, <mu, y>} rounded up.  A query (mu: the table's mean, v = q) writes {C0, C_ex, |A y|, K} from
+// these, |q|, <q, mu> and its sketch's norm and bound E_q (qsk, written before by sketch_rows_kernel):
+//   C0   = <q, mu> + g_c |q| |mu| + tiny - base,                     every quantity rounded up;
+//   C_ex = |p^_q| + E_q + s1 (E_q + g7 |p^_q|) + k (eps1 |q - mu| + g_c |q|),
+//   K    = |q| k, so that |q| |x| <= |q| |mu| + K ex_x;  +inf when |q| |mu| >= 2^125 (the screen keeps every id);
+// a query whose norm is not finite gets C0 = NaN, which keeps every id too.
+template <bool kQuery>
+__global__ void __launch_bounds__(256) dot_terms_kernel(const float* __restrict__ X, int64_t n, int dim, const float4* __restrict__ Pt4,
+                                                        const float* __restrict__ mu, DotConsts c, const float* __restrict__ qsk,
+                                                        float2* __restrict__ row_out, float4* __restrict__ q_out) {
+  const int lane = threadIdx.x & 31;
+  const int64_t i = static_cast<int64_t>(blockIdx.x) * 8 + (threadIdx.x >> 5);
+  if (i >= n) return;
+  const float* x = X + i * dim;
+  double w[kSketch];
+#pragma unroll
+  for (int j = 0; j < kSketch; ++j) w[j] = 0.0;
+  double yy = 0.0, my = 0.0, qq = 0.0, qm = 0.0;
+  for (int k = lane; k < dim; k += 32) {
+    const double xv = x[k], mv = mu[k], y = xv - mv;
+    yy = fma(y, y, yy);
+    my = fma(mv, y, my);
+    if (kQuery) { qq = fma(xv, xv, qq); qm = fma(xv, mv, qm); }
+#pragma unroll
+    for (int g = 0; g < kSketch / 4; ++g) {
+      const float4 p = __ldg(Pt4 + k * (kSketch / 4) + g);
+      w[4 * g] = fma(static_cast<double>(p.x), y, w[4 * g]);
+      w[4 * g + 1] = fma(static_cast<double>(p.y), y, w[4 * g + 1]);
+      w[4 * g + 2] = fma(static_cast<double>(p.z), y, w[4 * g + 2]);
+      w[4 * g + 3] = fma(static_cast<double>(p.w), y, w[4 * g + 3]);
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < kSketch; ++j)
+    for (int o = 16; o > 0; o >>= 1) w[j] += __shfl_xor_sync(kFull, w[j], o);
+  double rr = 0.0;
+  for (int k = lane; k < dim; k += 32) {
+    double r = static_cast<double>(x[k]) - static_cast<double>(mu[k]);
+#pragma unroll
+    for (int g = 0; g < kSketch / 4; ++g) {
+      const float4 p = __ldg(Pt4 + k * (kSketch / 4) + g);
+      r = fma(-static_cast<double>(p.x), w[4 * g], r);
+      r = fma(-static_cast<double>(p.y), w[4 * g + 1], r);
+      r = fma(-static_cast<double>(p.z), w[4 * g + 2], r);
+      r = fma(-static_cast<double>(p.w), w[4 * g + 3], r);
+    }
+    rr = fma(r, r, rr);
+  }
+  double pp = 0.0;  // query: |p^_q|^2, one sketch component per lane
+  if (kQuery) { const double p = qsk[i * kSketch + lane]; pp = p * p; }
+  for (int o = 16; o > 0; o >>= 1) {
+    yy += __shfl_xor_sync(kFull, yy, o);
+    my += __shfl_xor_sync(kFull, my, o);
+    rr += __shfl_xor_sync(kFull, rr, o);
+    if (kQuery) {
+      qq += __shfl_xor_sync(kFull, qq, o);
+      qm += __shfl_xor_sync(kFull, qm, o);
+      pp += __shfl_xor_sync(kFull, pp, o);
+    }
+  }
+  if (lane != 0) return;
+  const double up = 1.0 + (dim + 8) * 0x1.0p-52, yn = sqrt(yy) * up;
+  const double ay = (sqrt(rr) * up + yn * c.ay_rel) * (1.0 + 0x1.0p-50);
+  if (!kQuery) {
+    const double muy = my + (dim + 6) * 0x1.0p-52 * c.mu_norm * yn;
+    row_out[i] = make_float2(__double2float_ru(ay), __double2float_ru(muy + fabs(muy) * 0x1.0p-50));
+    return;
+  }
+  const double qn = sqrt(qq) * up, q1n = yn * (1.0 + 0x1.0p-52), qmu = qm + (dim + 6) * 0x1.0p-52 * qn * c.mu_norm;
+  const double pn = sqrt(pp) * (1.0 + 0x1.0p-45), eq = qsk[n * kSketch + i], qm_n = qn * c.mu_norm * (1.0 + 0x1.0p-50);
+  double c0 = qmu + c.g_c * qm_n + c.tiny;
+  c0 = c0 + fabs(c0) * 0x1.0p-50 - c.base;
+  c0 += fabs(c0) * 0x1.0p-50;
+  const double cex = (pn + eq + c.s1 * (eq + c.g7 * pn) + c.k * (c.eps1 * q1n + c.g_c * qn)) * (1.0 + 0x1.0p-40);
+  double kq = qn * c.k * (1.0 + 0x1.0p-50);
+  if (!(qm_n < 0x1.0p125)) kq = INFINITY;
+  if (!(qn <= DBL_MAX)) c0 = NAN;
+  q_out[i] = make_float4(__double2float_ru(c0), __double2float_ru(cex), __double2float_ru(ay), __double2float_ru(kq));
+}
+
+DotConsts dot_consts(const Index* ix) {
+  const int dim = static_cast<int>(ix->dim), m = kSketch, nc = 4 * ((dim + 127) / 128) + 5;
+  const double u = 0x1.0p-24, e = ix->sk_eps;
+  const double epn = std::sqrt(static_cast<double>(m)) * ((dim + 2) * u / (1.0 - (dim + 2) * u)) * std::sqrt(1.0 + e);  // as sketch_rows
+  DotConsts c;
+  c.ay_rel = ((1.0 + e) * (m + 2) * (dim + m + 6) * 0x1.0p-52 + std::max(1.0, e) * 0x1.0p-52) * (1.0 + 0x1.0p-40);
+  c.mu_norm = ix->sk_mu_norm;
+  c.k = (1.0 / epn) * (1.0 + (dim + 8) * 0x1.0p-52) * (1.0 + 0x1.0p-40);
+  c.s1 = (std::sqrt(1.0 + e) * c.k + 1.0) * (1.0 + 0x1.0p-40);
+  c.eps1 = e * (1.0 + e) * (1.0 + 0x1.0p-40);
+  c.g_c = nc * u / (1.0 - nc * u) * (1.0 + 0x1.0p-40);
+  c.g7 = 7 * u / (1.0 - 7 * u) * (1.0 + 0x1.0p-40);
+  c.tiny = (nc + 8) * 0x1.0p-149;
+  c.base = ix->metric == EPS_METRIC_COSINE ? 1.0 : 0.0;
+  return c;
+}
+
+template <bool kQuery>
+int launch_dot_terms(Index* ix, const float* d_x, int64_t n, const float* qsk, float2* row_out, float4* q_out) {
+  if (n <= 0) return EPS_OK;
+  const int dim = static_cast<int>(ix->dim);
+  dot_terms_kernel<kQuery><<<static_cast<unsigned>((n + 7) / 8), 256, 0, ix->stream>>>(
+      d_x, n, dim, ix->d_sk_basis.as<const float4>(), ix->d_sk_basis + static_cast<int64_t>(dim) * kSketch, dot_consts(ix), qsk,
+      row_out, q_out);
+  EPS_CUDA(cudaGetLastError());
+  return EPS_OK;
+}
+
 }  // namespace
 
 void free_sketch(Index* ix) {
@@ -173,9 +300,31 @@ int sketch_rows(Index* ix, const float* d_x, int64_t n, float* d_sk, float* d_ex
   return EPS_OK;
 }
 
+int dot_row_terms(Index* ix, const float* d_x, int64_t n, float2* d_terms) {
+  return launch_dot_terms<false>(ix, d_x, n, nullptr, d_terms, nullptr);
+}
+
+int sketch_queries(Index* ix, const float* d_q, int64_t nq, float* qsk, uint64_t* launches) {
+  EPS_TRY(sketch_rows(ix, d_q, nq, qsk, qsk + nq * kSketch));
+  ++*launches;
+  if (ix->metric == EPS_METRIC_L2) return EPS_OK;
+  EPS_TRY(launch_dot_terms<true>(ix, d_q, nq, qsk, nullptr, reinterpret_cast<float4*>(qsk + sk_qterms_off(nq))));
+  ++*launches;
+  return EPS_OK;
+}
+
+int64_t sketch_floats(const Index* ix, int64_t n) {
+  return ix->metric == EPS_METRIC_L2 ? n * (kSketch + 1) : sk_terms_off(n) + 2 * n;
+}
+
 bool screen_on(const Index* ix) {
-  return ix->metric == EPS_METRIC_L2 && ix->d_sk &&
+  return ix->d_sk &&
          (ix->graph_screen == EPS_GRAPH_SCREEN_ON || (ix->graph_screen == EPS_GRAPH_SCREEN_AUTO && ix->sk_share >= kScreenShare));
+}
+
+int screen_kind(const Index* ix) {
+  if (!screen_on(ix)) return kScreenNone;
+  return ix->metric == EPS_METRIC_L2 ? kScreenL2 : kScreenDot;
 }
 
 namespace {
@@ -212,14 +361,19 @@ int compute_sketch(Index* ix) {
     ix->sk_eps = eps;
     ix->sk_g = round_down(1.0 - gm);
     ix->sk_scale = round_down((1.0 - 2.0 * (dim + 2) * u) / (1.0 + eps));
+    double mu2 = 0.0;
+    for (int k = 0; k < dim; ++k) mu2 += static_cast<double>(mean[k]) * static_cast<double>(mean[k]);
+    ix->sk_mu_norm = std::sqrt(mu2) * (1.0 + (dim + 8) * 0x1.0p-52);
   }
   const bool want = ix->graph_screen == EPS_GRAPH_SCREEN_ON || ix->sk_share >= kScreenShare;
   if (!want) ix->d_sk.release();
 
   if (want && !ix->d_sk) {
     const int64_t n = ix->n_indexed;
-    EPS_TRY(ix->d_sk.reserve(static_cast<size_t>(n) * (m + 1) * 4));  // [n x m] sketches, then [n] bounds
+    EPS_TRY(ix->d_sk.reserve(static_cast<size_t>(sketch_floats(ix, n)) * 4));  // [n x m] sketches, [n] bounds (, [n] terms)
     EPS_TRY(sketch_rows(ix, ix->d_vectors, n, ix->d_sk, ix->d_sk + n * m));
+    if (ix->metric != EPS_METRIC_L2)
+      EPS_TRY(dot_row_terms(ix, ix->d_vectors, n, reinterpret_cast<float2*>(ix->d_sk + sk_terms_off(n))));
     EPS_CUDA(cudaStreamSynchronize(ix->stream));
   }
   return EPS_OK;
@@ -228,8 +382,7 @@ int compute_sketch(Index* ix) {
 }  // namespace
 
 void ensure_sketch(Index* ix) {
-  if (ix->metric != EPS_METRIC_L2 || ix->graph_screen == EPS_GRAPH_SCREEN_OFF || ix->dim < 128 || ix->n_indexed < 1 ||
-      !ix->d_vectors) {
+  if (ix->graph_screen == EPS_GRAPH_SCREEN_OFF || ix->dim < 128 || ix->n_indexed < 1 || !ix->d_vectors) {
     ix->d_sk.release();
     return;
   }

@@ -158,12 +158,14 @@ class Index:
         check(self.L.eps_index_set_graph_tuning(self.h, int(ring_slots), int(ctas_per_sm)))
 
     def set_graph_screen(self, mode):
-        """Graph-search screen of fresh neighbours on their 32-float principal-subspace sketch (L2; never changes
-        results): 0 = off, 1 = on, 2 = auto (on when the sketch's basis carries >= 90 % of the table's variance)."""
+        """Graph-search screen of fresh neighbours on their 32-float principal-subspace sketch (L2, inner product and
+        cosine; never changes results): 0 = off, 1 = on, 2 = auto (on when the sketch's basis carries >= 90 % of the
+        table's variance)."""
         check(self.L.eps_index_set_graph_screen(self.h, int(mode)))
 
     def graph_screen_info(self):
-        """dict(active=bool, share=explained-variance share of the basis or -1, n_screened=ids dropped so far)."""
+        """dict(active=bool, share=explained-variance share of the basis (any metric) or -1 when there is no basis,
+        n_screened=ids dropped so far)."""
         act, share, n = C.c_int(0), C.c_double(0.0), C.c_uint64(0)
         check(self.L.eps_index_graph_screen_info(self.h, C.byref(act), C.byref(share), C.byref(n)))
         return dict(active=bool(act.value), share=float(share.value), n_screened=int(n.value))

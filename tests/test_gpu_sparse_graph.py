@@ -152,6 +152,27 @@ def test_sparse_graph_bitmap_fallback(vdb, port):
     ix.close()
 
 
+def test_sparse_graph_bitmap_touched_words_clear(vdb, port):
+    """L = 64 on 640 000 short rows: every query evaluates more rows than the 768 inserts its 1024-entry hash set
+    allows, so it moves to the bitmap, and ten times its rows stay under the bitmap's 20 000 words, so the clean-up
+    clears only the words it touched.  A word left dirty would change the second search."""
+    n, vocab, nq, L = 640_000, 64, 4, 64
+    rows = sparse_rows(n, vocab, 73, max_nnz=4)
+    qs = sparse_rows(nq, vocab, 74, max_nnz=6, empty_every=0, dup_every=0)
+    D = ref_distances(densify(rows, vocab), densify(qs, vocab), L2)
+    ix = vdb.SparseIndex("l2", vocab)
+    ix.append(rows)
+    ix.build(n, out_degree=50)
+    graph = ix.get_graph()
+    ix.set_search_mode(GRAPH)
+    n_dist = port_model(port, D, graph, L, 10)[3]  # per query; check() holds the device's total to their sum
+    assert (n_dist > 768).all(), "n_dist per query %s: not every query moved to the bitmap" % n_dist
+    assert (10 * n_dist < (n + 31) // 32).all(), "n_dist per query %s: the bitmap is cleared whole" % n_dist
+    for run in (1, 2):
+        check(ix, port, qs, D, graph, L, 10, "touched-words clear, search %d" % run)
+    ix.close()
+
+
 def test_sparse_graph_branch_rule(vdb):
     n, vocab, nq = 3000, 2000, 8
     rows = sparse_rows(n, vocab, 81)

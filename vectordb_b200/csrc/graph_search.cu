@@ -28,12 +28,10 @@
 //     while the FIFO has a backlog; accepted keys (key < worst-in-queue) go to a small pending buffer that is merged
 //     into the sorted queue by a block-parallel rank-and-shift, at the latest when the expansion is consumed;
 //   * adjacency: fixed-stride rows of 64 int32 ids (one 256-byte read from the vertex id; longer rows
-//     continue in the CSR); visited: a per-slot open-addressing hash set of int32 ids in global memory (16 L entries,
-//     at most 64 KB: the tables of all resident queries fit in L2), one 32-byte bucket read + atomicCAS per
-//     test-and-insert, refilled with 0xFF after the query like the reference clears its vector<bool> (:711-714).  A
-//     query that would fill the set beyond 3/4 moves to a bitmap of n bits (atomicOr test-and-set) for the rest of
-//     its run; that bitmap is cleared after the query — on large tables only the words the query touched, from a log
-//     of its fresh ids.
+//     continue in the CSR); visited: the per-slot visited set of graph_search.cuh, shared with the sparse kernel (its
+//     rules are written there): a hash set in L2 with one 32-byte bucket read + atomicCAS per test-and-insert, a
+//     bitmap for queries that outgrow it, left clean after the query like the reference clears its vector<bool>
+//     (:711-714).
 //   * screen (sketch.cu; L2, and inner product / cosine through a bound on the dot product): once the queue holds L
 //     entries, the fresh ids of a step are checked against a proven lower bound from 32-float principal-subspace
 //     sketches of the row and the query, and only those it cannot reject enter
@@ -389,14 +387,10 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
       unsigned long long key = kKeyInf;
       if (i < L) {
         const uint32_t id = static_cast<uint32_t>(a.init_ids[i]);
-        if (hashed) {
-          vset_claim(vset, vmask, vset_bucket(id, a.vset_shift), id, vacc);
+        visit_seed(vset, vmask, a.vset_shift, visited, hashed, id, vacc);
 #ifdef EPS_GS_PROFILE
-          ++prof_vtest;
+        if (hashed) ++prof_vtest;
 #endif
-        } else {
-          atomicOr(&visited[id >> 5], 1u << (id & 31));
-        }
         key = make_key(a.seed_dist[static_cast<int64_t>(q) * a.seed_ld + i], id);
       }
       qa[i] = key;
@@ -404,8 +398,7 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
     if (tid == 0) { s_npend = 0; s_ncont = 0; s_cursor = 0; s_ncur = 0; s_head = 0u; }
     __syncthreads();
     block_bitonic_sort(qa, a.Lp);
-    for (int w = tid; w < ((L + 31) >> 5); w += kGsThreads)  // every seed starts unchecked
-      ubits[w] = (w * 32 + 32 <= L) ? 0xffffffffu : ((1u << (L & 31)) - 1u);
+    init_unchecked(ubits, L);
     if (kCollect) {  // the list starts with the first cap passing seeds of the sorted queue
       if (warp == 0) {
         int n = 0;
@@ -526,22 +519,7 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
           unsigned long long pmin = ~0ull;  // smallest unchecked pending key
           bool pscan = np > 0;
           while (cnt < W) {
-            int qpos = -1;
-            {
-              const int nwords = (L + 31) >> 5;
-              for (int w0 = sp >> 5; w0 < nwords; w0 += 32) {
-                const int wi = w0 + lane;
-                unsigned word = wi < nwords ? ubits[wi] : 0u;
-                if (wi == (sp >> 5)) word &= ~((1u << (sp & 31)) - 1u);  // entries before the cursor are checked
-                const unsigned b = __ballot_sync(kFull, word != 0u);
-                if (b) {
-                  const int src = __ffs(b) - 1;
-                  const unsigned wsel = __shfl_sync(kFull, word, src);
-                  qpos = (w0 + src) * 32 + __ffs(wsel) - 1;
-                  break;
-                }
-              }
-            }
+            const int qpos = first_unchecked(ubits, L, sp, lane);
             if (qpos < 0) sp = L;  // queue exhausted: later picks of this iteration do not rescan it
             const unsigned long long qkey = qpos >= 0 ? (qa[qpos] & kKeyMask) : ~0ull;
             if (pscan) {
@@ -602,19 +580,10 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
         e0 = s_cont_e[ncont - 1];
         nslots = static_cast<int>(min(static_cast<long long>(kGsThreads), s_cont_end[ncont - 1] - e0));
       }
-      // a step inserts at most nslots ids: move to the bitmap before the hash set could pass 3/4 full.  Every id the
-      // query has visited is a seed or in the log (fifo_tail <= vset_max < vlog_cap).  Block-uniform.
+      // a step inserts at most nslots ids (visited-set rules: graph_search.cuh).  Block-uniform.
       if (hashed && L + fresh_tail() + static_cast<uint32_t>(nslots) > static_cast<uint32_t>(a.vset_max)) {
-        for (int i = tid; i < L; i += kGsThreads) {
-          const uint32_t id = static_cast<uint32_t>(a.init_ids[i]);
-          atomicOr(&visited[id >> 5], 1u << (id & 31));
-        }
-        for (uint32_t i = tid; i < fresh_tail(); i += kGsThreads) {
-          const uint32_t id = static_cast<uint32_t>(vlog[i]);
-          atomicOr(&visited[id >> 5], 1u << (id & 31));
-        }
+        move_to_bitmap(a.init_ids, L, vlog, fresh_tail(), visited);
         hashed = false;
-        __syncthreads();  // every bit is set before any thread tests one
       }
       int nb[kRounds];
       unsigned bal[kRounds];
@@ -628,24 +597,13 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
       }
       // test-and-insert (ExpandOneCandidate :403-406); of two slots racing on one id exactly one finds it fresh
       if (hashed) {
-        // one bucket read per id: an entry equal to it = visited; else a CAS on the first free entry of the bucket (the
-        // next bucket's first entry when it is full), and a CAS lost to another id goes on probing entry by entry
+        // every bucket read of the step, then every CAS, then the claims of the lost CASes
         uint32_t at[kRounds], old[kRounds];
 #pragma unroll
         for (int r = 0; r < kRounds; ++r) {
           at[r] = kVsetEmpty;
           if (nb[r] >= 0) {
-            const uint32_t id = static_cast<uint32_t>(nb[r]), b = vset_bucket(id, a.vset_shift);
-            const uint4 lo = __ldcg(reinterpret_cast<const uint4*>(vset + b)), hi = __ldcg(reinterpret_cast<const uint4*>(vset + b) + 1);
-            const uint32_t e[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
-            bool hit = false;
-            uint32_t fe = 8;
-#pragma unroll
-            for (int j = 7; j >= 0; --j) {
-              hit |= e[j] == id;
-              if (e[j] == kVsetEmpty) fe = j;
-            }
-            if (!hit) at[r] = (b + fe) & vmask;
+            at[r] = vset_probe(vset, vmask, a.vset_shift, static_cast<uint32_t>(nb[r]));
 #ifdef EPS_GS_PROFILE
             ++prof_vtest; ++vacc;
 #endif
@@ -660,8 +618,7 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
 #ifdef EPS_GS_PROFILE
             ++vacc;
 #endif
-            const uint32_t id = static_cast<uint32_t>(nb[r]);
-            fr[r] = old[r] == kVsetEmpty || (old[r] != id && vset_claim(vset, vmask, (at[r] + 1) & vmask, id, vacc));
+            fr[r] = vset_settle(vset, vmask, at[r], old[r], static_cast<uint32_t>(nb[r]), vacc);
           }
         }
       } else {
@@ -777,27 +734,10 @@ __global__ void __launch_bounds__(kGsThreads, kMinCtas) graph_search_kernel(GSAr
       a.qtimes[4 * q + 1] = t; a.qtimes[4 * q + 2] = st_ndist - prof_nd0; a.qtimes[4 * q + 3] = prof_iters;
     }
 #endif
-    // the hash set: 16-byte stores over the whole table (at most 64 KB, in L2); the bitmap only if the query moved to it
-    {
-      uint4* t4 = reinterpret_cast<uint4*>(vset);
-      const uint4 e = make_uint4(kVsetEmpty, kVsetEmpty, kVsetEmpty, kVsetEmpty);
-      for (int i = tid; i < (a.vset_cap >> 2); i += kGsThreads) t4[i] = e;
-    }
 #ifdef EPS_GS_PROFILE
     if (tid == 0 && !hashed) ++prof_migrated;
 #endif
-    if (hashed) continue;
-    if (fresh_tail() <= static_cast<uint32_t>(a.vlog_cap) && 10ll * (fresh_tail() + L) < a.visited_words) {
-      // large table: clear only the words this query touched (the seeds and the logged fresh ids) instead of
-      // streaming zeros over the whole bitmap (1.25 MB per query at 10M rows)
-      for (int i = tid; i < L; i += kGsThreads) visited[static_cast<uint32_t>(a.init_ids[i]) >> 5] = 0u;
-      for (uint32_t i = tid; i < fresh_tail(); i += kGsThreads) visited[static_cast<uint32_t>(vlog[i]) >> 5] = 0u;
-    } else {
-      uint4* v4 = reinterpret_cast<uint4*>(visited);
-      const int64_t n4 = a.visited_words >> 2;
-      const uint4 z = make_uint4(0, 0, 0, 0);
-      for (int64_t i = tid; i < n4; i += kGsThreads) v4[i] = z;
-    }
+    reset_visited(vset, a.vset_cap, hashed, visited, a.visited_words, a.init_ids, L, vlog, fresh_tail());
   }
 #ifdef EPS_GS_PROFILE
   if (lane == 0 && warp < 2) {
@@ -1075,20 +1015,16 @@ int prepare_visited(Index* ix, int slots, int64_t L, VisitedSets* v) {
     ix->visited_gen = ix->s_visited.gen;
     ix->visited_words = words;
   }
-  // Visited hash sets: 16 entries per queue slot, so that the ~10 L ids a query visits load its table about 2/3 (a
-  // query that needs more moves to its bitmap), and at most 16384 entries = 64 KB per slot: the tables of the 528
-  // queries resident at the benchmark's geometry take 34 MB of the 50 MB L2.  The kernel refills every table it
-  // touched, so the whole buffer is all-ones between launches whatever the table size; fill it when it is (re)allocated.
-  const int vset_cap = std::min(16384, std::max(1024, next_pow2(16 * static_cast<int>(L))));
+  // Hash sets (sizes and rules: graph_search.cuh).  The kernel refills every table it touched, so the whole buffer is
+  // all-ones between launches whatever the table size; fill it when it is (re)allocated.
+  const int vset_cap = vset_cap_for(L);
   EPS_TRY(ix->s_vset.reserve(static_cast<size_t>(slots) * vset_cap * 4));
   if (ix->vset_gen != ix->s_vset.gen) {
     EPS_CUDA(cudaMemsetAsync(ix->s_vset.p, 0xff, ix->s_vset.cap, ix->stream));
     ix->vset_gen = ix->s_vset.gen;
   }
-  // fresh ids of the running query in FIFO order: the migration to the bitmap and the bitmap reset read them
-  constexpr int kVlogCap = 32768;
   EPS_TRY(ix->s_vlog.reserve(static_cast<size_t>(slots) * kVlogCap * 4));
-  v->vset = ix->s_vset.as<uint32_t>(); v->vset_cap = vset_cap; v->vset_max = vset_cap / 4 * 3;
+  v->vset = ix->s_vset.as<uint32_t>(); v->vset_cap = vset_cap; v->vset_max = vset_max_for(vset_cap);
   v->vset_shift = 32 - (__builtin_ctz(static_cast<unsigned>(vset_cap)) - 3);
   v->visited = ix->s_visited.as<uint32_t>(); v->words = words;
   v->vlog = ix->s_vlog.as<int32_t>(); v->vlog_cap = kVlogCap;

@@ -15,8 +15,8 @@
 //     kSgQCap; a longer query is read from global memory) live in shared memory;
 //   * adjacency: straight from the CSR in chunks of 128 ids (sparse graphs have long navigation rows: the build's
 //     repair adds its component entries there), one id per thread;
-//   * visited: the dense kernel's per-slot hash set in L2 (graph_search.cuh), moving to the per-slot bitmap when the
-//     query would fill it beyond 3/4; fresh ids are compacted in adjacency order and logged for the migration / reset;
+//   * visited: the per-slot visited set of graph_search.cuh, shared with the dense kernel (its rules are written
+//     there); fresh ids are compacted in adjacency order and logged;
 //   * distances: one thread per fresh row feeds the row to a SparseMerge against the staged query (a row's fp32 sum is
 //     a serial chain whichever way the work is split; 128 chains run side by side); keys below the worst queue entry
 //     go to the pending buffer;
@@ -53,26 +53,6 @@ struct SGArgs {
   unsigned long long* stats;      // counter block (GraphCounter slots)
   int L, Lp, nq;
 };
-
-// Test-and-insert of one id into the hash set: one 32-byte bucket read; an entry equal to the id = visited; else a CAS
-// on the first free entry of the bucket (the next bucket's first entry when it is full), and a CAS lost to another id
-// goes on probing entry by entry (the dense kernel's step, one id per thread).  True when this thread inserted it.
-__device__ __forceinline__ bool vset_test_insert(uint32_t* vset, uint32_t vmask, int shift, uint32_t id, unsigned long long& acc) {
-  const uint32_t b = vset_bucket(id, shift);
-  const uint4 lo = __ldcg(reinterpret_cast<const uint4*>(vset + b)), hi = __ldcg(reinterpret_cast<const uint4*>(vset + b) + 1);
-  const uint32_t e[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
-  bool hit = false;
-  uint32_t fe = 8;
-#pragma unroll
-  for (int j = 7; j >= 0; --j) {
-    hit |= e[j] == id;
-    if (e[j] == kVsetEmpty) fe = j;
-  }
-  if (hit) return false;
-  const uint32_t at = (b + fe) & vmask;
-  const uint32_t old = atomicCAS(vset + at, kVsetEmpty, id);
-  return old == kVsetEmpty || (old != id && vset_claim(vset, vmask, (at + 1) & vmask, id, acc));
-}
 
 template <int METRIC>
 __global__ void __launch_bounds__(kGsThreads) sparse_graph_search_kernel(SGArgs a) {
@@ -117,8 +97,7 @@ __global__ void __launch_bounds__(kGsThreads) sparse_graph_search_kernel(SGArgs 
       unsigned long long key = kKeyInf;
       if (i < L) {
         const uint32_t id = static_cast<uint32_t>(a.init_ids[i]);
-        if (hashed) vset_claim(vset, vmask, vset_bucket(id, a.vset_shift), id, vacc);
-        else atomicOr(&visited[id >> 5], 1u << (id & 31));
+        visit_seed(vset, vmask, a.vset_shift, visited, hashed, id, vacc);
         key = make_key(sparse_row_dist<METRIC>(a.row_ptr, a.elems, a.row_norm2, id, qv, qn_el, qn), id);
       }
       qa[i] = key;
@@ -126,8 +105,7 @@ __global__ void __launch_bounds__(kGsThreads) sparse_graph_search_kernel(SGArgs 
     if (tid == 0) { s_npend = 0; s_cursor = 0; }
     __syncthreads();
     block_bitonic_sort(qa, a.Lp);
-    for (int w = tid; w < ((L + 31) >> 5); w += kGsThreads)  // every seed starts unchecked
-      ubits[w] = (w * 32 + 32 <= L) ? 0xffffffffu : ((1u << (L & 31)) - 1u);
+    init_unchecked(ubits, L);
     if (tid == 0) st_ndist += static_cast<unsigned long long>(L);
     uint32_t n_fresh = 0;  // fresh ids of this query so far (block-uniform)
 
@@ -136,21 +114,7 @@ __global__ void __launch_bounds__(kGsThreads) sparse_graph_search_kernel(SGArgs 
       __syncthreads();  // the previous expansion is merged; every thread has read s_cid
       // pick: the first unchecked entry at or after the cursor (warp 0)
       if (warp == 0) {
-        const int sp = s_cursor;
-        const int nwords = (L + 31) >> 5;
-        int qpos = -1;
-        for (int w0 = sp >> 5; w0 < nwords; w0 += 32) {
-          const int wi = w0 + lane;
-          unsigned word = wi < nwords ? ubits[wi] : 0u;
-          if (wi == (sp >> 5)) word &= ~((1u << (sp & 31)) - 1u);  // entries before the cursor are not looked at
-          const unsigned b = __ballot_sync(kFull, word != 0u);
-          if (b) {
-            const int src = __ffs(b) - 1;
-            const unsigned wsel = __shfl_sync(kFull, word, src);
-            qpos = (w0 + src) * 32 + __ffs(wsel) - 1;
-            break;
-          }
-        }
+        const int qpos = first_unchecked(ubits, L, s_cursor, lane);
         if (lane == 0) {
           if (qpos >= 0) {
             qa[qpos] |= kCheckedBit;
@@ -169,26 +133,18 @@ __global__ void __launch_bounds__(kGsThreads) sparse_graph_search_kernel(SGArgs 
       const int64_t e1 = a.offsets[c + 1];
       for (int64_t e = a.offsets[c]; e < e1; e += kGsThreads) {
         const int nslots = static_cast<int>(min(static_cast<int64_t>(kGsThreads), e1 - e));
-        // a chunk inserts at most nslots ids: move to the bitmap before the hash set could pass 3/4 full.  Every id the
-        // query has visited is a seed or in the log (n_fresh <= vset_max < vlog_cap).  Block-uniform.
+        // a chunk inserts at most nslots ids (visited-set rules: graph_search.cuh).  Block-uniform.
         if (hashed && static_cast<uint32_t>(L) + n_fresh + static_cast<uint32_t>(nslots) > static_cast<uint32_t>(a.vset_max)) {
-          for (int i = tid; i < L; i += kGsThreads) {
-            const uint32_t id = static_cast<uint32_t>(a.init_ids[i]);
-            atomicOr(&visited[id >> 5], 1u << (id & 31));
-          }
-          for (uint32_t i = tid; i < n_fresh; i += kGsThreads) {
-            const uint32_t id = static_cast<uint32_t>(vlog[i]);
-            atomicOr(&visited[id >> 5], 1u << (id & 31));
-          }
+          move_to_bitmap(a.init_ids, L, vlog, n_fresh, visited);
           hashed = false;
-          __syncthreads();  // every bit is set before any thread tests one
         }
         // test-and-insert (ExpandOneCandidate :403-406); of two slots racing on one id exactly one finds it fresh
         const int nb = tid < nslots ? __ldg(a.nbrs + e + tid) : -1;
         bool fr = false;
         if (nb >= 0) {
           if (hashed) {
-            fr = vset_test_insert(vset, vmask, a.vset_shift, static_cast<uint32_t>(nb), vacc);
+            const uint32_t id = static_cast<uint32_t>(nb), at = vset_probe(vset, vmask, a.vset_shift, id);
+            fr = at != kVsetEmpty && vset_settle(vset, vmask, at, atomicCAS(vset + at, kVsetEmpty, id), id, vacc);
           } else {
             const uint32_t bit = 1u << (nb & 31);
             fr = !(atomicOr(&visited[nb >> 5], bit) & bit);
@@ -230,22 +186,7 @@ __global__ void __launch_bounds__(kGsThreads) sparse_graph_search_kernel(SGArgs 
     // ---- results + visited reset (:711-714) ----
     unsigned long long* out = a.out_queue + static_cast<int64_t>(q) * L;
     for (int i = tid; i < L; i += kGsThreads) out[i] = qa[i];
-    {
-      uint4* t4 = reinterpret_cast<uint4*>(vset);
-      const uint4 e = make_uint4(kVsetEmpty, kVsetEmpty, kVsetEmpty, kVsetEmpty);
-      for (int i = tid; i < (a.vset_cap >> 2); i += kGsThreads) t4[i] = e;
-    }
-    if (hashed) continue;
-    if (n_fresh <= static_cast<uint32_t>(a.vlog_cap) && 10ll * (n_fresh + L) < a.visited_words) {
-      // large table: clear only the words this query touched
-      for (int i = tid; i < L; i += kGsThreads) visited[static_cast<uint32_t>(a.init_ids[i]) >> 5] = 0u;
-      for (uint32_t i = tid; i < n_fresh; i += kGsThreads) visited[static_cast<uint32_t>(vlog[i]) >> 5] = 0u;
-    } else {
-      uint4* v4 = reinterpret_cast<uint4*>(visited);
-      const int64_t n4 = a.visited_words >> 2;
-      const uint4 z = make_uint4(0, 0, 0, 0);
-      for (int64_t i = tid; i < n4; i += kGsThreads) v4[i] = z;
-    }
+    reset_visited(vset, a.vset_cap, hashed, visited, a.visited_words, a.init_ids, L, vlog, n_fresh);
   }
 #ifdef EPS_GS_PROFILE
   if (vacc) atomicAdd(&a.stats[kGcVsetAccesses], vacc);

@@ -428,7 +428,8 @@ EPS_API int eps_index_set_sparse_search(eps_index* ix, int mode);
  * index order from 0, in fp32 without FMA, as the merge adds them (db/vector.cpp:7-47), so the distances are bitwise
  * those of the scan: ids, distances, counts and the n_dist / n_seed / n_expand / n_edges counters are what they are
  * without the index.  Only kernel_launches and the timings change.
- * Appends: rows appended after the build are scanned until the caller builds again, the way the graph's tail is.
+ * Appends: rows appended after the build are scanned until the caller builds again or extends the lists
+ * (eps_index_extend_sparse_postings), the way the graph's tail is.
  * n = 0 drops the index.  A build replaces the previous index only once it has succeeded; a refused or failed call
  * leaves the previous index as it was.  Refusals: an L2 index, EPS_ERR_UNSUPPORTED (its merged order also adds the
  * row-only and query-only terms); a null or dense index, n < 0, n above the mirrored rows, a view, or an index with live
@@ -459,7 +460,8 @@ EPS_API int eps_index_sparse_inverted_info(eps_index* ix, int64_t* n_rows, int64
  * (each a sequential sum with a known error bound) and m_r, every step rounded toward -inf (sparse_inverted.cu
  * restates the derivation).  Rows with a non-finite |row|^2 (NaN or +-inf values, squares that overflow), pairs with
  * m + 2 > 2^20, and every row for a query with a non-finite |q|^2 are always re-scored.
- * Lifecycle as for the inverted index: rows appended after the build are merged until the next build; n = 0 drops the
+ * Lifecycle as for the inverted index: rows appended after the build are merged until the caller builds again or
+ * extends the lists (eps_index_extend_sparse_postings); n = 0 drops the
  * lists; a refused or failed call leaves the previous state; views created after the build share it.  Refusals, all
  * EPS_ERR_INVALID_ARGUMENT: a null or dense index, an inner-product or cosine index (eps_index_build_sparse_inverted
  * gives those exact distances from the same lists), n < 0, n above the mirrored rows, a view, or an index with live
@@ -469,6 +471,31 @@ EPS_API int eps_index_build_sparse_l2_screen(eps_index* ix, int64_t n);
  * handle's searches and builds have re-scored through the merge so far; waits for the index's stream.  Any pointer may
  * be NULL.  A null or dense index: EPS_ERR_INVALID_ARGUMENT. */
 EPS_API int eps_index_sparse_l2_screen_info(eps_index* ix, int64_t* n_rows, uint64_t* n_rescored);
+
+/* Extend the posting lists of a sparse index (the inverted index of an IP or cosine index, the L2 screen of an L2 one)
+ * over the rows [inv_rows, n) appended since they were built, without rebuilding them.  Afterwards the lists are,
+ * byte for byte, those eps_index_build_sparse_inverted(ix, n) or eps_index_build_sparse_l2_screen(ix, n) would make
+ * (deleted rows included, as the builds include them), so every search and graph build reads them as it would after
+ * that build.  Only the appended rows' postings are sorted; the old postings keep their order and are copied once to
+ * their place in the new arrays.  n == the covered rows does nothing and returns EPS_OK.  The call synchronises the
+ * index's stream and does not touch the count of re-scored pairs.
+ * Refusals, all EPS_ERR_INVALID_ARGUMENT and all leaving the lists as they were: a null or dense index, an index
+ * without posting lists (build them first), n below the covered rows (a build with a smaller n shrinks them), n above
+ * the mirrored rows, a view, or an index with live views.  A failed allocation or launch also leaves the previous lists
+ * in place: the new ones are installed only once every step has succeeded.
+ * Device memory while it runs, with P_old / T_old the postings / distinct indices of the lists, P_new / T_new those of
+ * the appended rows and T the distinct indices after: the new lists, 8 B x (P_old + P_new) + 12 B x T + 8 B, beside the
+ * old ones, which are freed when the new ones are installed; the appended rows' sort, 24 B x P_new plus the sort's
+ * scratch, of which 8 B x P_new stay until the merge; and 28 B x T_new + 8 B x T_old of term bookkeeping plus a scan's
+ * scratch.  A rebuild instead needs 24 B x (P_old + P_new) plus the sort's scratch beside the old lists. */
+EPS_API int eps_index_extend_sparse_postings(eps_index* ix, int64_t n);
+/* Copy the posting lists out, as eps_index_get_graph copies the graph: n_rows = the rows covered, then n_terms
+ * distinct indices (terms, ascending), their n_terms + 1 offsets (ptr, from 0 to n_postings), and the postings split
+ * into their rows and values (term terms[t] holds rows[ptr[t] .. ptr[t+1]), ascending, with their values).  Pass NULL
+ * buffers to query the sizes.  An index without lists gives zeros and writes no buffer.  A null or dense index:
+ * EPS_ERR_INVALID_ARGUMENT. */
+EPS_API int eps_index_get_sparse_postings(eps_index* ix, int64_t* n_rows, int64_t* n_terms, int64_t* n_postings,
+                                          uint32_t* terms, int64_t* ptr, int32_t* rows, float* values);
 
 /* Raw stream handle (cudaStream_t) the index launches on, for callers that time with CUDA events. */
 EPS_API void* eps_index_stream(eps_index* ix);

@@ -931,6 +931,48 @@ int eps_index_build_sparse_l2_screen(eps_index* h, int64_t n) {
   return eps::build_sparse_inverted(ix, n);
 }
 
+int eps_index_extend_sparse_postings(eps_index* h, int64_t n) {
+  Index* ix = reinterpret_cast<Index*>(h);
+  if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");
+  if (!ix->sparse) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "posting lists on a dense index");
+  EPS_TRY(check_mutable(ix));
+  if (ix->inv_rows == 0)
+    return eps::fail(EPS_ERR_INVALID_ARGUMENT, "extend_sparse_postings: no posting lists (build them first with "
+                                               "eps_index_build_sparse_inverted or eps_index_build_sparse_l2_screen)");
+  if (n < ix->inv_rows) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "extend_sparse_postings: n below the covered rows");
+  if (n > ix->n_rows) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "extend_sparse_postings: n above the mirrored rows");
+  if (n == ix->inv_rows) return EPS_OK;
+  EPS_TRY(eps::check_device(ix->device));
+  return eps::extend_sparse_inverted(ix, n);
+}
+
+int eps_index_get_sparse_postings(eps_index* h, int64_t* n_rows, int64_t* n_terms, int64_t* n_postings, uint32_t* terms,
+                                  int64_t* ptr, int32_t* rows, float* values) {
+  Index* ix = reinterpret_cast<Index*>(h);
+  if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");
+  if (!ix->sparse) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "posting lists of a dense index");
+  if (n_rows) *n_rows = ix->inv_rows;
+  if (n_terms) *n_terms = ix->inv_terms;
+  if (n_postings) *n_postings = ix->inv_postings;
+  if (ix->inv_rows == 0 || !(terms || ptr || rows || values)) return EPS_OK;
+  EPS_TRY(eps::check_device(ix->device));
+  if (terms && ix->inv_terms > 0)
+    EPS_CUDA(cudaMemcpyAsync(terms, ix->d_inv_terms, static_cast<size_t>(ix->inv_terms) * 4, cudaMemcpyDeviceToHost, ix->stream));
+  if (ptr)
+    EPS_CUDA(cudaMemcpyAsync(ptr, ix->d_inv_ptr, static_cast<size_t>(ix->inv_terms + 1) * 8, cudaMemcpyDeviceToHost, ix->stream));
+  std::vector<uint2> post;
+  if ((rows || values) && ix->inv_postings > 0) {
+    post.resize(static_cast<size_t>(ix->inv_postings));
+    EPS_CUDA(cudaMemcpyAsync(post.data(), ix->d_inv_post, post.size() * 8, cudaMemcpyDeviceToHost, ix->stream));
+  }
+  EPS_CUDA(cudaStreamSynchronize(ix->stream));
+  for (size_t i = 0; i < post.size(); ++i) {  // {row, value bits} pairs
+    if (rows) rows[i] = static_cast<int32_t>(post[i].x);
+    if (values) std::memcpy(&values[i], &post[i].y, 4);
+  }
+  return EPS_OK;
+}
+
 int eps_index_sparse_l2_screen_info(eps_index* h, int64_t* n_rows, uint64_t* n_rescored) {
   Index* ix = reinterpret_cast<Index*>(h);
   if (!ix) return eps::fail(EPS_ERR_INVALID_ARGUMENT, "null index");

@@ -286,6 +286,9 @@ int build_graph_sparse(Index* ix, int64_t n, const eps_build_params* params);
 // ---- sparse_inverted.cu --------------------------------------------------------------------
 // Posting lists of rows [0, n) of a sparse index (n = 0 drops them); the caller has validated ix and n.
 int build_sparse_inverted(Index* ix, int64_t n);
+// The posting lists extended over rows [inv_rows, n), to the arrays build_sparse_inverted(ix, n) makes; the caller has
+// validated ix and inv_rows < n <= n_rows.
+int extend_sparse_inverted(Index* ix, int64_t n);
 // The sparse scan's distance tile with the rows [0, inv_rows) read from the posting lists, bitwise the tile of
 // SparseDist: each row's products are added in the query's index order, from 0, as sparse_dist_kernel adds them.
 // Rows at or above inv_rows go to SparseDist.  The queries' elements are [elem_base, elem_base + n_elems) of q.elems

@@ -18,6 +18,11 @@
 // flags (term slots), then scatter the terms and their offsets.  The new arrays replace the old ones only when every
 // step has succeeded.
 //
+// Extension (eps_index_extend_sparse_postings): rows [inv_rows, n) are sorted the same way on their own, and the two
+// lists are merged term by term: each old term's block moves, unchanged, to its place in the union, and the new rows'
+// postings follow it.  Old postings are copied once and never sorted again; the arrays are the full build's, bit for
+// bit (extend_sparse_inverted).
+//
 // Search: once per call, inverted_plan_kernel maps every query element to its posting range (binary search on the
 // terms; an index no covered row has gets an empty range).  inverted_score_kernel: one CTA = one query x a slice of
 // kInvSlice rows with their accumulators in shared memory.  Per batch of up to kInvThreads terms, one thread per term
@@ -41,17 +46,19 @@ namespace {
 constexpr int kInvSlice = 2048;   // rows per CTA: 8 KB of accumulators; 1M rows give one query 489 CTAs
 constexpr int kInvThreads = 256;  // threads per CTA = terms whose bounds one pass finds
 
-// One warp per row: element p of row r becomes the pair (index, {r, value bits}) at position p (row_ptr[0] = 0).
-__global__ void inverted_expand_kernel(const int64_t* __restrict__ row_ptr, const uint2* __restrict__ elems, int64_t n,
-                                       uint32_t* __restrict__ keys, uint2* __restrict__ vals) {
-  const int64_t r = (blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5;
+// One warp per row of [row_base, n): element p of row r becomes the pair (index, {r, value bits}) at position
+// p - elem_base (elem_base = row_ptr[row_base]).
+__global__ void inverted_expand_kernel(const int64_t* __restrict__ row_ptr, const uint2* __restrict__ elems,
+                                       int64_t row_base, int64_t elem_base, int64_t n, uint32_t* __restrict__ keys,
+                                       uint2* __restrict__ vals) {
+  const int64_t r = row_base + ((blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x) >> 5);
   const int lane = threadIdx.x & 31;
   if (r >= n) return;
   const int64_t p1 = row_ptr[r + 1];
   for (int64_t p = row_ptr[r] + lane; p < p1; p += 32) {
     const uint2 e = elems[p];
-    keys[p] = e.x;
-    vals[p] = make_uint2(static_cast<uint32_t>(r), e.y);
+    keys[p - elem_base] = e.x;
+    vals[p - elem_base] = make_uint2(static_cast<uint32_t>(r), e.y);
   }
 }
 
@@ -76,6 +83,79 @@ __global__ void inverted_scatter_kernel(const uint32_t* __restrict__ keys, int64
     terms[slot[i]] = keys[i];
     ptr[slot[i]] = i;
   }
+}
+
+// First i of [0, len) with a[i] >= x (a ascending).
+__device__ __forceinline__ int64_t terms_lower_bound(const uint32_t* a, int64_t len, uint32_t x) {
+  int64_t lo = 0, hi = len;
+  while (lo < hi) {
+    const int64_t m = lo + ((hi - lo) >> 1);
+    if (a[m] < x) lo = m + 1;
+    else hi = m;
+  }
+  return lo;
+}
+
+__device__ __forceinline__ bool has_term(const uint32_t* a, int64_t len, int64_t i, uint32_t x) {
+  return i < len && a[i] == x;
+}
+
+// Extension, step 1 (one thread per term j of the appended rows, plus one): only[j] = 1 when no old term equals new
+// term j, only[t_new] = 0.  Their exclusive sum is, at j, the new-only terms below new term j and, at t_new, their number.
+__global__ void extend_probe_kernel(const uint32_t* __restrict__ old_terms, int64_t t_old,
+                                    const uint32_t* __restrict__ new_terms, int64_t t_new, int64_t* __restrict__ only) {
+  const int64_t j = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (j > t_new) return;
+  only[j] = j < t_new && !has_term(old_terms, t_old, terms_lower_bound(old_terms, t_old, new_terms[j]), new_terms[j]);
+}
+
+// Step 2 (one thread per old term, then one per new term, plus one): the union's terms, ascending, and each one's
+// posting count in count[0, t), count[t] = 0.  Old term i goes to slot i + (new-only terms below it); new term j to slot
+// (old terms below it) + below[j], where an old term with the same index is.  A shared term is counted by its new term.
+__global__ void extend_union_kernel(const uint32_t* __restrict__ old_terms, const int64_t* __restrict__ old_ptr,
+                                    int64_t t_old, const uint32_t* __restrict__ new_terms,
+                                    const int64_t* __restrict__ new_ptr, int64_t t_new, const int64_t* __restrict__ below,
+                                    int64_t* __restrict__ old_slot, int64_t* __restrict__ new_slot,
+                                    uint32_t* __restrict__ terms, int64_t* __restrict__ count, int64_t t) {
+  const int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (i < t_old) {
+    const uint32_t x = old_terms[i];
+    const int64_t j = terms_lower_bound(new_terms, t_new, x);
+    const int64_t s = i + below[j];
+    old_slot[i] = s;
+    terms[s] = x;
+    if (!has_term(new_terms, t_new, j, x)) count[s] = old_ptr[i + 1] - old_ptr[i];
+  } else if (i < t_old + t_new) {
+    const int64_t j = i - t_old;
+    const uint32_t x = new_terms[j];
+    const int64_t o = terms_lower_bound(old_terms, t_old, x);
+    const int64_t s = o + below[j];
+    new_slot[j] = s;
+    int64_t c = new_ptr[j + 1] - new_ptr[j];
+    if (has_term(old_terms, t_old, o, x)) c += old_ptr[o + 1] - old_ptr[o];
+    else terms[s] = x;
+    count[s] = c;
+  } else if (i == t_old + t_new) {
+    count[t] = 0;
+  }
+}
+
+// Step 3 (one thread per posting p of one source: the old lists, or the appended rows' sorted postings): p's term i is
+// the last one whose offset is <= p (every term has a posting, so src_ptr ascends strictly).  The old postings open
+// their union term's block, in their order; the new ones close it, in theirs.
+__global__ void extend_place_kernel(const uint2* __restrict__ src, const int64_t* __restrict__ src_ptr, int64_t t_src,
+                                    int64_t p_src, const int64_t* __restrict__ slot, bool at_end,
+                                    const int64_t* __restrict__ ptr, uint2* __restrict__ post) {
+  const int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+  if (p >= p_src) return;
+  int64_t lo = 0, hi = t_src - 1;
+  while (lo < hi) {
+    const int64_t m = hi - ((hi - lo) >> 1);
+    if (src_ptr[m] <= p) lo = m;
+    else hi = m - 1;
+  }
+  const int64_t d = at_end ? ptr[slot[lo] + 1] - src_ptr[lo + 1] : ptr[slot[lo]] - src_ptr[lo];
+  post[p + d] = src[p];
 }
 
 // plan[e] = the posting range of query element e's index, or an empty range when no covered row has it.
@@ -263,19 +343,23 @@ __global__ void __launch_bounds__(kL2Threads) l2_rescore_kernel(
 
 unsigned blocks_for(int64_t threads, int per_block) { return static_cast<unsigned>((threads + per_block - 1) / per_block); }
 
-}  // namespace
+// Posting lists of some rows, laid out as the index's: terms ascending, offsets, postings with rows ascending per term.
+struct Postings {
+  DevArray<uint32_t> terms;  // [T]
+  DevArray<int64_t> ptr;     // [T + 1]
+  DevArray<uint2> post;      // [P]
+  int64_t T = 0, P = 0;
+};
 
-int build_sparse_inverted(Index* ix, int64_t n) {
-  if (n == 0) {
-    ix->d_inv_terms.release();
-    ix->d_inv_ptr.release();
-    ix->d_inv_post.release();
-    ix->inv_rows = ix->inv_terms = ix->inv_postings = 0;
-    return EPS_OK;
-  }
-  int64_t P = 0;
-  EPS_CUDA(cudaMemcpyAsync(&P, ix->d_sp_ptr + n, 8, cudaMemcpyDeviceToHost, ix->stream));
+// The posting lists of rows [r0, n): expand them to (index, {row, value}) pairs, sort the pairs by index with a stable
+// radix sort (rows stay ascending within a term), flag the first posting of each term, take the int64 exclusive sum of
+// the flags (term slots), then scatter the terms and their offsets.  Offsets count from the first posting of row r0.
+int sort_postings(Index* ix, int64_t r0, int64_t n, Postings* out) {
+  int64_t e[2] = {0, 0};  // element offsets of rows r0 and n
+  EPS_CUDA(cudaMemcpyAsync(&e[0], ix->d_sp_ptr + r0, 8, cudaMemcpyDeviceToHost, ix->stream));
+  EPS_CUDA(cudaMemcpyAsync(&e[1], ix->d_sp_ptr + n, 8, cudaMemcpyDeviceToHost, ix->stream));
   EPS_CUDA(cudaStreamSynchronize(ix->stream));
+  const int64_t P = e[1] - e[0];
   // indices are < dim: the sort looks at the bits of dim - 1 only
   int bits = 1;
   while (bits < 32 && ((static_cast<uint64_t>(ix->dim) - 1) >> bits) != 0) ++bits;
@@ -288,7 +372,8 @@ int build_sparse_inverted(Index* ix, int64_t n) {
   EPS_TRY(keys_b.reserve(std::max<size_t>(P, 1) * 4));
   EPS_TRY(vals_a.reserve(P1 * 8));
   EPS_TRY(vals_b.reserve(P1 * 8));
-  inverted_expand_kernel<<<blocks_for(n * 32, 256), 256, 0, ix->stream>>>(ix->d_sp_ptr, ix->d_sp_elems, n, keys_a, vals_a);
+  inverted_expand_kernel<<<blocks_for((n - r0) * 32, 256), 256, 0, ix->stream>>>(ix->d_sp_ptr, ix->d_sp_elems, r0, e[0], n,
+                                                                                 keys_a, vals_a);
   EPS_CUDA(cudaGetLastError());
   cub::DoubleBuffer<uint32_t> kb(keys_a, keys_b);
   cub::DoubleBuffer<uint64_t> vb(reinterpret_cast<uint64_t*>(vals_a.p), reinterpret_cast<uint64_t*>(vals_b.p));
@@ -313,13 +398,90 @@ int build_sparse_inverted(Index* ix, int64_t n) {
   inverted_scatter_kernel<<<blocks_for(P + 1, 256), 256, 0, ix->stream>>>(kb.Current(), P, flags, terms, ptr);
   EPS_CUDA(cudaGetLastError());
   EPS_CUDA(cudaStreamSynchronize(ix->stream));
-  // every step succeeded: install (the previous arrays go out with the temporaries)
-  ix->d_inv_terms.swap(terms);
-  ix->d_inv_ptr.swap(ptr);
-  ix->d_inv_post.swap(post);
+  out->terms.swap(terms);
+  out->ptr.swap(ptr);
+  out->post.swap(post);
+  out->T = T;
+  out->P = P;
+  return EPS_OK;
+}
+
+// Every step succeeded: the lists replace the index's (whose arrays go out with `l`).
+void install(Index* ix, Postings* l, int64_t n) {
+  ix->d_inv_terms.swap(l->terms);
+  ix->d_inv_ptr.swap(l->ptr);
+  ix->d_inv_post.swap(l->post);
   ix->inv_rows = n;
-  ix->inv_terms = T;
-  ix->inv_postings = P;
+  ix->inv_terms = l->T;
+  ix->inv_postings = l->P;
+}
+
+}  // namespace
+
+int build_sparse_inverted(Index* ix, int64_t n) {
+  if (n == 0) {
+    ix->d_inv_terms.release();
+    ix->d_inv_ptr.release();
+    ix->d_inv_post.release();
+    ix->inv_rows = ix->inv_terms = ix->inv_postings = 0;
+    return EPS_OK;
+  }
+  Postings l;
+  EPS_TRY(sort_postings(ix, 0, n, &l));
+  install(ix, &l, n);
+  return EPS_OK;
+}
+
+// The lists of rows [inv_rows, n) are sorted on their own and merged into the index's: the union of the two term sets
+// (extend_probe_kernel, its exclusive sum, extend_union_kernel), the union's offsets (the exclusive sum of its counts),
+// then every old posting and every new one copied to its place (extend_place_kernel).  The new rows are numbered above
+// every covered row, so appending them to their terms' blocks gives each block the order a stable sort of [0, n) gives
+// it: the arrays are those build_sparse_inverted(ix, n) makes.
+int extend_sparse_inverted(Index* ix, int64_t n) {
+  Postings add;
+  EPS_TRY(sort_postings(ix, ix->inv_rows, n, &add));
+  if (add.P == 0) {  // empty rows only: the lists do not change
+    ix->inv_rows = n;
+    return EPS_OK;
+  }
+  const int64_t t_old = ix->inv_terms, p_old = ix->inv_postings;
+  DevArray<int64_t> below, old_slot, new_slot;
+  DevBuf tmp;
+  EPS_TRY(below.reserve(static_cast<size_t>(add.T + 1) * 8));
+  EPS_TRY(old_slot.reserve(static_cast<size_t>(std::max<int64_t>(t_old, 1)) * 8));
+  EPS_TRY(new_slot.reserve(static_cast<size_t>(add.T) * 8));
+  extend_probe_kernel<<<blocks_for(add.T + 1, 256), 256, 0, ix->stream>>>(ix->d_inv_terms, t_old, add.terms, add.T, below);
+  EPS_CUDA(cudaGetLastError());
+  size_t scan_bytes = 0;
+  EPS_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, below.as<int64_t>(), add.T + 1, ix->stream));
+  EPS_TRY(tmp.reserve(scan_bytes));
+  EPS_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, scan_bytes, below.as<int64_t>(), add.T + 1, ix->stream));
+  int64_t only = 0;
+  EPS_CUDA(cudaMemcpyAsync(&only, below + add.T, 8, cudaMemcpyDeviceToHost, ix->stream));
+  EPS_CUDA(cudaStreamSynchronize(ix->stream));
+  Postings all;
+  all.T = t_old + only;
+  all.P = p_old + add.P;
+  EPS_TRY(all.terms.reserve(static_cast<size_t>(all.T) * 4));
+  EPS_TRY(all.ptr.reserve(static_cast<size_t>(all.T + 1) * 8));
+  EPS_TRY(all.post.reserve(static_cast<size_t>(all.P) * 8));
+  extend_union_kernel<<<blocks_for(t_old + add.T + 1, 256), 256, 0, ix->stream>>>(
+      ix->d_inv_terms, ix->d_inv_ptr, t_old, add.terms, add.ptr, add.T, below, old_slot, new_slot, all.terms, all.ptr,
+      all.T);
+  EPS_CUDA(cudaGetLastError());
+  EPS_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, all.ptr.as<int64_t>(), all.T + 1, ix->stream));
+  EPS_TRY(tmp.reserve(scan_bytes));
+  EPS_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, scan_bytes, all.ptr.as<int64_t>(), all.T + 1, ix->stream));
+  if (p_old > 0) {
+    extend_place_kernel<<<blocks_for(p_old, 256), 256, 0, ix->stream>>>(ix->d_inv_post, ix->d_inv_ptr, t_old, p_old,
+                                                                         old_slot, false, all.ptr, all.post);
+    EPS_CUDA(cudaGetLastError());
+  }
+  extend_place_kernel<<<blocks_for(add.P, 256), 256, 0, ix->stream>>>(add.post, add.ptr, add.T, add.P, new_slot, true,
+                                                                       all.ptr, all.post);
+  EPS_CUDA(cudaGetLastError());
+  EPS_CUDA(cudaStreamSynchronize(ix->stream));
+  install(ix, &all, n);
   return EPS_OK;
 }
 

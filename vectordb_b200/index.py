@@ -256,7 +256,8 @@ class SparseIndex(Index):
     scans by default; set_search_mode("graph") searches the graph that build() installed where the reference would
     (n_indexed >= 512, no prefilter / force_brute), with the reference's results at IntraQueryThreads = 1.
     build_inverted() gives an IP or cosine index posting lists that the exact scans read, and build_l2_screen() gives an
-    L2 index posting lists that screen the exact scans' rows with a proven lower bound, both with the same results.  Config,
+    L2 index posting lists that screen the exact scans' rows with a proven lower bound, both with the same results;
+    extend_postings() extends either over appended rows without a rebuild, and postings() copies them out.  Config,
     deleted bits, attributes, string codes and dictionary, facets, build and get_graph work as on Index."""
 
     def __init__(self, metric, dim, capacity=0, device=0):
@@ -274,7 +275,7 @@ class SparseIndex(Index):
     def build_inverted(self, n=None):
         """Posting lists of rows [0, n) (None: every mirrored row; 0 drops them) for an IP or cosine index
         (eps_index_build_sparse_inverted).  Results do not change; the exact scans read the covered rows' distances
-        from the postings.  Rows appended later are scanned until the next build."""
+        from the postings.  Rows appended later are scanned until the next build or extend_postings()."""
         check(self.L.eps_index_build_sparse_inverted(self.h, self.rows if n is None else int(n)))
 
     def inverted_info(self):
@@ -287,7 +288,7 @@ class SparseIndex(Index):
         """Posting lists of rows [0, n) (None: every mirrored row; 0 drops them) for an L2 index
         (eps_index_build_sparse_l2_screen).  Results do not change; the exact scans and the build's kNN pass re-score
         only the covered rows whose proven lower bound can still place them among the k best.  Rows appended later are
-        merged until the next build."""
+        merged until the next build or extend_postings()."""
         check(self.L.eps_index_build_sparse_l2_screen(self.h, self.rows if n is None else int(n)))
 
     def l2_screen_info(self):
@@ -295,6 +296,25 @@ class SparseIndex(Index):
         r, c = C.c_int64(0), C.c_uint64(0)
         check(self.L.eps_index_sparse_l2_screen_info(self.h, C.byref(r), C.byref(c)))
         return dict(rows=int(r.value), rescored=int(c.value))
+
+    def extend_postings(self, n=None):
+        """Extend the posting lists (the inverted index or the L2 screen) over the rows appended since they were built,
+        up to row n (None: every mirrored row), without rebuilding them (eps_index_extend_sparse_postings).  The lists
+        are then those a build over [0, n) makes."""
+        check(self.L.eps_index_extend_sparse_postings(self.h, self.rows if n is None else int(n)))
+
+    def postings(self):
+        """The posting lists (eps_index_get_sparse_postings): dict(rows=rows covered, terms=distinct indices ascending
+        (uint32), ptr=their offsets (int64, terms + 1 of them), post_rows=rows (int32), ascending within a term,
+        post_values=values (float32))."""
+        r, t, p = C.c_int64(0), C.c_int64(0), C.c_int64(0)
+        check(self.L.eps_index_get_sparse_postings(self.h, C.byref(r), C.byref(t), C.byref(p), None, None, None, None))
+        terms = np.zeros(t.value, np.uint32)
+        ptr = np.zeros(t.value + 1, np.int64)
+        rows = np.zeros(p.value, np.int32)
+        values = np.zeros(p.value, np.float32)
+        check(self.L.eps_index_get_sparse_postings(self.h, None, None, None, _p(terms), _p(ptr), _p(rows), _p(values)))
+        return dict(rows=int(r.value), terms=terms, ptr=ptr, post_rows=rows, post_values=values)
 
     def append(self, rows, first_row=None):
         """Append CSR rows (scipy CSR or (offsets, indices, values)) after the rows already mirrored."""

@@ -11,7 +11,8 @@ EXPORTS = [
     "eps_index_set_graph", "eps_index_build", "eps_index_extend_graph", "eps_index_get_graph", "eps_index_set_deleted", "eps_index_set_attrs", "eps_index_set_string_codes", "eps_index_append_string_dictionary",
     "eps_index_config", "eps_index_set_coarse", "eps_index_set_coarse_guard", "eps_index_set_search_width", "eps_index_set_filter_search", "eps_index_set_graph_tuning", "eps_index_set_graph_screen", "eps_index_graph_screen_info", "eps_search_batch", "eps_search_batch_device", "eps_merge_shards_device", "eps_facet_batch", "eps_shard_unique_id", "eps_shard_group_create", "eps_shard_group_destroy", "eps_search_batch_sharded", "eps_normalize",
     "eps_pair_distances", "eps_index_stream", "eps_index_create_sparse", "eps_index_append_sparse_rows", "eps_search_sparse_batch", "eps_index_set_sparse_search", "eps_index_build_sparse_inverted", "eps_index_sparse_inverted_info",
-    "eps_index_build_sparse_l2_screen", "eps_index_sparse_l2_screen_info", "eps_last_error", "eps_version", "eps_device_count",
+    "eps_index_build_sparse_l2_screen", "eps_index_sparse_l2_screen_info", "eps_index_extend_sparse_postings",
+    "eps_index_get_sparse_postings", "eps_last_error", "eps_version", "eps_device_count",
 ]
 
 
@@ -112,6 +113,8 @@ def load_library():
     L.eps_index_sparse_inverted_info.argtypes = [vp, vp, vp, vp]
     L.eps_index_build_sparse_l2_screen.argtypes = [vp, i64]
     L.eps_index_sparse_l2_screen_info.argtypes = [vp, vp, vp]
+    L.eps_index_extend_sparse_postings.argtypes = [vp, i64]
+    L.eps_index_get_sparse_postings.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp]
     L.eps_index_stream.argtypes = [vp]
     L.eps_index_stream.restype = vp
     L.eps_last_error.restype = C.c_char_p
